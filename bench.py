@@ -2,8 +2,9 @@
 """bench.py -- Nexmark-shaped streaming HashJoin (headline) and HashAgg (secondary) throughput.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--legs value,e2e,agg,chain,cpu]
+                    [--dump-outputs DIR]
 
-Workload (BASELINE.json configs[2], "Nexmark q7/q8 streaming HashJoin (bid x auction) 1xB200, 10M build
+Workload (BASELINE.json configs[2], "Nexmark q7/q8 streaming HashJoin (bid x auction) 1xH100, 10M build
 rows in HBM"; SURVEY 8(d) cfg3):  the auction side (10 000 000 rows: id, seller, category, expires)
 is loaded into the right-side join state, then every STEP pushes one batch of 2^20 bid rows
 (auction, date_time, bidder, price; 1024 StreamChunks of 1024 rows coalesced into one device batch)
@@ -21,10 +22,12 @@ RWGPU_EXCHANGE=nccl selects partition + NCCL all-to-all-v instead.
             per rank, no exchange).
 `secondary`: BASELINE configs[1] (q4-shaped HashAgg: count(*), sum, max GROUP BY auction, 2^18-row epochs).
 `chain`   : join -> Filter -> Project -> HashAgg without leaving HBM (SURVEY 8(f) rank 1), a barrier per batch.
-`roofline`: dominant kernel, algorithmic bytes / CUDA-event time against MEASURED_PEAKS.json; `traffic` from the
-            committed ncu capture (profiles/r1_traffic.json).  `clocks`: in-process NVML samples during the region.
+`roofline`: dominant kernel, algorithmic bytes / CUDA-event time against MEASURED_PEAKS.json when present, else the
+            H100 SXM data-sheet HBM3 bandwidth.  `clocks`: in-process NVML samples during the region.
 `--impl reference`: the CPU restatement of the reference algorithm (oracle/fastcpu.cc, one
 single-threaded actor per host core, inputs pre-partitioned by vnode) on a bounded sample.
+`--dump-outputs DIR`: after the timed steps, the join output of the last timed step of `value` (rank 0), canonically
+ordered, as DIR/<name>.npy (see dump_join_output).  Inputs are seeded: the same arguments give the same inputs.
 """
 import argparse
 import contextlib
@@ -242,16 +245,6 @@ def pin_to_gpu_numa_node(gpu_index):
         pass
 
 
-def ncu_traffic(kernel):
-    """DRAM bytes per launch of `kernel` from the committed ncu captures (profiles/r2_traffic.json, r1_traffic.json), or None"""
-    for f in ("r2_traffic.json", "r1_traffic.json"):
-        try:
-            return float(json.load(open(os.path.join(ROOT, "profiles", f)))[kernel]["bytes_per_launch"])
-        except Exception:
-            continue
-    return None
-
-
 def bench_config(world):
     """the `config` object of the JSON line -- key-identical in both arms (the driver compares them)"""
     return {"workload": "nexmark_q7q8_hashjoin_cfg3" if world == 1 else "nexmark_q8_shuffled_hashjoin_cfg4",
@@ -265,7 +258,7 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s; not a measured peak)"
 
 
 # ------------------------------------------------------------------------------------------ CPU arm
@@ -438,6 +431,33 @@ def cpu_join_run(auct, batches, cpu_ids, warmup, chunk=CHUNK, pin=True, after=No
 
 
 # ------------------------------------------------------------------------------------------ GPU arm
+JOIN_OUT_NAMES = ("bid_auction", "bid_date_time", "bid_bidder", "bid_price",
+                  "auction_id", "auction_seller", "auction_category", "auction_expires")
+DUMP_MAX_ROWS = 1 << 19  # 9 arrays x 2^19 rows x 8 bytes = 36 MiB
+
+
+def dump_join_output(view, out_dir):
+    """--dump-outputs: the last timed step's join output as DIR/<name>.npy.  The visible rows are put in a canonical order
+    (sorted by every column, then the op) because the kernel emits them in no fixed order; above DUMP_MAX_ROWS rows a fixed,
+    seeded sample of that order is kept.  Columns are float64 (every value of this workload is an integer below 2^53, so
+    exactly representable), ops float32; `rows.npy` holds the visible row count before sampling."""
+    ops = view.ops().cpu().numpy()
+    cols = [view.column(k).cpu().numpy() for k in range(len(JOIN_OUT_NAMES))]
+    vis = view.visible()
+    if vis is not None:
+        vis = vis.cpu().numpy()
+        ops, cols = ops[vis], [c[vis] for c in cols]
+    order = np.lexsort([ops] + cols[::-1])
+    n = len(order)
+    if n > DUMP_MAX_ROWS:
+        order = order[np.sort(np.random.default_rng(SEED).choice(n, DUMP_MAX_ROWS, replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "rows.npy"), np.array([n], np.float64))
+    np.save(os.path.join(out_dir, "ops.npy"), ops[order].astype(np.float32))
+    for name, c in zip(JOIN_OUT_NAMES, cols):
+        np.save(os.path.join(out_dir, name + ".npy"), c[order].astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -599,12 +619,15 @@ def run_ours(args):
                 keep[s] = ch  # the input buffers stay alive until the push is collected
                 device.join_push_device_async(join, abi.SIDE_LEFT, ch, stream)
 
+            last_out = [None]  # the most recently collected output view (read by --dump-outputs after the timed steps)
+
             def collect(s):
                 nonlocal t_join
                 tb = time.perf_counter()
                 out = device.join_collect(join, stream)
                 t_join += time.perf_counter() - tb
                 keep.pop(s, None)
+                last_out[0] = out
                 return out
 
             tl = []  # BENCH_TRACE: host timeline (never for a reported number)
@@ -647,6 +670,8 @@ def run_ours(args):
             if world > 1:
                 dist.barrier()
             ms = e0.elapsed_time(e1)
+            if args.dump_outputs and rank == 0:  # (before the verification pushes reuse the view's output set)
+                dump_join_output(last_out[0], args.dump_outputs)
             if trace:
                 print("[trace] step: launch ms, collect(prev) ms\n" + "\n".join(f"  {a}: {b:.3f} {c:.3f}" for a, b, c in tl[-K:]), file=sys.stderr)
             clocks = sampler.stop() if rank == 0 else None
@@ -674,7 +699,7 @@ def run_ours(args):
                 "build_rows_per_s": world / build_s, "build_first_push_ms": build_first_ms[0], "out_rows": out_rows, "gpu_launches": int(launches), "clocks": clocks,
                 "roofline": {"bound": "hbm", "kernel": "uni_hot_kernel<false,false,4> (unified bucket: probe + emit + own-side append, 4 lanes per row)",
                              "achieved": fused_gbs, "peak": peak, "unit": "GB/s", "frac": fused_gbs / peak if fused_gbs else None,
-                             "traffic": ncu_traffic("uni_hot_kernel"), "traffic_unit": "bytes per launch (ncu dram read+write)",
+                             "traffic": None,
                              "algorithmic_bytes_per_launch": JOIN_BYTES_PER_ROW_STEP * BATCH,
                              "peak_source": which, "algorithmic_bytes_per_row": JOIN_BYTES_PER_ROW_STEP,
                              "rows_per_launch": BATCH, "kernel_ms_avg": kern_ms / max(kern_n, 1),
@@ -967,7 +992,7 @@ def run_ours(args):
                 "verified": bool((vr, vc) == (want_rows, want_cs)),
                 "verification": {"epochs": n_v, "gpu_delta_rows": vr, "cpu_delta_rows": want_rows, "gpu_checksum": f"{vc:016x}", "cpu_checksum": f"{want_cs:016x}"},
                 "roofline": {"bound": "hbm", "kernel": f"agg_apply_fast_kernel<{len(calls)}>", "achieved": agbs, "peak": peak, "unit": "GB/s",
-                             "frac": agbs / peak if agbs else None, "traffic": ncu_traffic("agg_apply_fast_kernel"), "peak_source": which,
+                             "frac": agbs / peak if agbs else None, "traffic": None, "peak_source": which,
                              "algorithmic_bytes_per_row": AGG_BYTES_PER_ROW_FLOOR, "kernel_ms_avg": akern_ms / max(akern_n, 1)},
                 "epoch_roofline": {"what": "apply + barrier delta together (the whole epoch), bytes incl. the emitted delta rows",
                                    "algorithmic_bytes_per_row": bpr, "achieved": step_gbs, "peak": peak, "unit": "GB/s", "frac": step_gbs / peak}}
@@ -1260,8 +1285,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--legs", default="value,retract,hot,e2e,agg,q1,chain,generic,cpu",
-                    help="comma list of: value,retract,hot,e2e,agg,q1,chain,generic,cpu (subset for ncu runs; retract needs value)")
+                    help="comma list of: value,retract,hot,e2e,agg,q1,chain,generic,cpu (retract needs value)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the join output of the last timed step (leg `value`) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "ours" or "value" not in args.legs.split(",")):
+        ap.error("--dump-outputs needs --impl ours and the `value` leg")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
     # stdout carries exactly ONE line (the JSON): everything a library prints there on its own (NCCL's "NCCL version ..."
     # banner at communicator creation, for one) is sent to stderr for the duration of the run

@@ -1,5 +1,5 @@
 /*
- * rwgpu.h -- C ABI of the B200-native streaming HashAgg / HashJoin / hash-shuffle path.
+ * rwgpu.h -- C ABI of the H100-native streaming HashAgg / HashJoin / hash-shuffle path.
  *
  * The reference (risingwavelabs/risingwave) has NO extern "C" surface on this path: the
  * operators are Rust types behind `trait Execute` (src/stream/src/executor/mod.rs:240-253)
@@ -490,7 +490,7 @@ int32_t rwgpu_project_device(const rw_chunk* chunk, const rw_project_expr* exprs
 const char* rwgpu_last_error(void);
 /* 0 if a CUDA device is usable, else RW_ERR_NO_DEVICE (and every create() fails loudly). */
 int32_t rwgpu_device_check(void);
-/* "rwgpu <version> sm_100a" */
+/* "rwgpu <version> sm_90a" */
 const char* rwgpu_version(void);
 
 #ifdef __cplusplus

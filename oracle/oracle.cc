@@ -13,11 +13,11 @@
 // into tests/golden/*.json.  The reference itself is Rust and cannot be compiled here (no
 // cargo/rustc), so there is no oracle/_ref.
 //
-// Third-party arithmetic not in /root/reference: CRC32 = crc32fast 1.5.0 (standard IEEE 802.3,
+// Third-party arithmetic not in the reference tree: CRC32 = crc32fast 1.5.0 (standard IEEE 802.3,
 // reflected 0xEDB88320, init/xorout 0xFFFFFFFF), restated below and cross-checked against zlib.
 // XxHash64 values are never observable in operator output and are not restated.
 //
-// Every function cites the reference file:line it follows (paths relative to /root/reference).
+// Every function cites the reference file:line it follows (paths relative to the reference checkout).
 //
 // Exposes the same C structs as include/rwgpu.h under the `rwo_` prefix.
 #include <algorithm>

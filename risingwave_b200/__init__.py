@@ -1,4 +1,4 @@
-"""risingwave_b200 -- B200-native (sm_100a) streaming HashAgg / HashJoin / hash-shuffle path behind
+"""risingwave_b200 -- H100-native (sm_90a) streaming HashAgg / HashJoin / hash-shuffle path behind
 RisingWave's executor interface.  See DESIGN.md for scope; include/rwgpu.h is the drop-in C ABI."""
 from . import abi  # noqa: F401
 from .stream_chunk import StreamChunk, Column  # noqa: F401

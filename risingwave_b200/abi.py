@@ -1,4 +1,4 @@
-"""ctypes mirror of include/rwgpu.h (the C ABI of the B200 HashAgg / HashJoin / shuffle path).
+"""ctypes mirror of include/rwgpu.h (the C ABI of the H100 HashAgg / HashJoin / shuffle path).
 
 The structs here are a 1:1 transcription of the header; `load_library()` loads the in-tree
 `librwgpu.so` and FAILS LOUDLY when it is missing -- there is no CPU fallback in the product.
@@ -121,7 +121,7 @@ def load_library() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback.")
+                "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.")
         _lib = C.CDLL(LIB_PATH)
     return _lib
 

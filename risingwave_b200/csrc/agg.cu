@@ -1,4 +1,4 @@
-// agg.cu -- streaming HashAgg on sm_100a: fused group-by hash + atomic partial aggregate, and the
+// agg.cu -- streaming HashAgg on sm_90a: fused group-by hash + atomic partial aggregate, and the
 // barrier-time delta (change inference + compaction) kernel.
 //
 // Replaces (reference, Rust):
@@ -328,8 +328,8 @@ __global__ void __launch_bounds__(256) agg_mm_delete_kernel(AggTable t, AggPlanD
 // Two rows per thread with 128-bit loads of the key / argument columns.
 // One atomic per BLOCK and loop round reserves the dirty-list entries of the block's first-touched groups, one per
 // block at the end counts the new groups: an atomicAdd per warp on those two shared counters (the first version)
-// serialised in one L2 slice -- ~8 K same-address atomics per 2^18-row epoch at one per ~7 cycles were the
-// kernel's whole duration.
+// serialised in one L2 slice -- thousands of same-address atomics per 2^18-row epoch made up the kernel's
+// whole duration.
 template <int NCALLS>
 __global__ void __launch_bounds__(256) agg_apply_fast_kernel(AggTable t, AggPlanDev p, DevChunk ch) {
   __shared__ unsigned int s_warp[8];
@@ -538,7 +538,7 @@ __device__ __forceinline__ void agg_publish(AggStatus* st, unsigned int* has_nul
 // The group's hot and cold rows are STAGED IN SHARED MEMORY: every word is fetched once by independent loads issued
 // back to back, the generic per-call logic below then runs on the staged copy, and the rows go back with one pass
 // of stores.  (Working on the global rows serialised ~20 dependent L2 round trips per thread -- the stores between the
-// loads keep the compiler from batching them: r2b ncu, 56 us per 2^18-row epoch at 15 % SM / 11 % DRAM.)
+// loads keep the compiler from batching them, leaving both SM and DRAM mostly idle.)
 __global__ void __launch_bounds__(256) agg_flush_kernel(AggTable t, AggPlanDev p, AggOutDev o, uint32_t epoch_flag_mask, AggPublish pub) {
   extern __shared__ uint64_t s_rows[];
   const int s_stride = (p.HW + p.CW) | 1;  // odd: conflict-free for 8-byte words
@@ -1081,7 +1081,7 @@ struct rwgpu_agg {
 
 static int grid_for(int64_t n_threads, int block) {
   int64_t g = (n_threads + block - 1) / block;
-  int64_t maxg = 148 * 8;
+  int64_t maxg = RW_SMS * 8;
   return (int)std::max<int64_t>(1, std::min(g, maxg));
 }
 

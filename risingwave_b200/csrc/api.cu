@@ -10,8 +10,8 @@ namespace rw {
 // driver entry points of the virtual memory management API, resolved once through the runtime
 static VmmApi load_vmm_api() {
   VmmApi a;
-  // opt-in: on the B200 boxes measured (profiles/README.md) cuMemCreate+cuMemMap of a few hundred MB took
-  // 8-11 ms, cudaMalloc + device copy + cudaFree of the same store 0.3-0.7 ms
+  // opt-in: cuMemCreate + cuMemMap of a few hundred MB can take longer than cudaMalloc + device copy + cudaFree of
+  // the same store
   if (!getenv("RWGPU_VMM")) return a;
   auto get = [](const char* name, void** fn) -> bool {
     cudaDriverEntryPointQueryResult q;
@@ -183,7 +183,7 @@ extern "C" {
 
 int32_t rwgpu_type_width(int32_t type) { return rw::type_is_varlen(type) ? 0 : rw::type_width(type); }
 const char* rwgpu_last_error(void) { return rw::last_error_cstr(); }
-const char* rwgpu_version(void) { return "rwgpu 0.1.0 sm_100a"; }
+const char* rwgpu_version(void) { return "rwgpu 0.1.0 sm_90a"; }
 
 int32_t rwgpu_device_check(void) {
   int n = 0;
@@ -198,7 +198,7 @@ int32_t rwgpu_device_check(void) {
   int dev = 0;
   cudaGetDevice(&dev);
   if (applied_dev != dev) {
-    size_t g = 0;  // default: leave the driver's 64 B (measured: 32 / 128 slow the build side 4-7x, steady state unchanged)
+    size_t g = 0;  // default: leave the driver's 64 B
     if (const char* v = getenv("RWGPU_L2_FETCH")) g = (size_t)atoi(v);
     if (g == 32 || g == 64 || g == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, g);
     cudaGetLastError();

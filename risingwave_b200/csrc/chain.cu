@@ -126,7 +126,7 @@ static int filter_launch(const FilterPlanDev& p, const DevChunk& ch, uint8_t* ou
   if (n_visible_dev) RW_CUDA(cudaMemsetAsync(n_visible_dev, 0, sizeof(int64_t), st));
   if (ch.n == 0) return RW_OK;
   const int64_t blocks = (ch.n + 255) / 256;
-  filter_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(blocks, 148 * 8)), 256, 0, st>>>(p, ch, out_ops, (uint32_t*)out_vis,
+  filter_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(blocks, RW_SMS * 8)), 256, 0, st>>>(p, ch, out_ops, (uint32_t*)out_vis,
                                                                                                    (unsigned long long*)n_visible_dev);
   RW_CUDA(cudaGetLastError());
   return RW_OK;
@@ -298,7 +298,7 @@ int32_t rwgpu_project_device(const rw_chunk* c, const rw_project_expr* exprs, in
   for (int e = 0; e < n_exprs; e++) { o.data[e] = out_data[e]; o.valid[e] = out_valid_bytes[e]; }
   o.has_null = has_null;
   const int64_t blocks = (ch.n + 255) / 256;
-  project_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(blocks, 148 * 8)), 256, 0, st>>>(p, ch, o);
+  project_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(blocks, RW_SMS * 8)), 256, 0, st>>>(p, ch, o);
   RW_CUDA(cudaGetLastError());
   return RW_OK;
 }
@@ -341,14 +341,14 @@ int32_t rwgpu_project(const rw_chunk* c, const rw_project_expr* exprs, int32_t n
     o.has_null = (unsigned int*)(d + o_flags);
     RW_CUDA(cudaMemset(d + o_flags, 0, sizeof(uint32_t) * PROJ_MAX_EXPRS));
     const int64_t blocks = (n + 255) / 256;
-    project_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(blocks, 148 * 8)), 256>>>(p, ch, o);
+    project_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(blocks, RW_SMS * 8)), 256>>>(p, ch, o);
     RW_CUDA(cudaGetLastError());
   }
   RW_CUDA(cudaMemcpy(has_null, d + o_flags, sizeof(uint32_t) * n_exprs, cudaMemcpyDeviceToHost));
   for (int e = 0; e < n_exprs; e++) {
     RW_CUDA(cudaMemcpy(out_data[e], dd[e], (size_t)n * p.ret_width[e], cudaMemcpyDeviceToHost));
     if (has_null[e] && out_validity[e]) {
-      pack_bytes_to_bits_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>((n + 63) / 64 / 256 + 1, 148 * 8)), 256>>>(dv[e], (uint64_t*)(d + o_bits[e]), n);
+      pack_bytes_to_bits_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>((n + 63) / 64 / 256 + 1, RW_SMS * 8)), 256>>>(dv[e], (uint64_t*)(d + o_bits[e]), n);
       RW_CUDA(cudaGetLastError());
       RW_CUDA(cudaMemcpy(out_validity[e], d + o_bits[e], nw, cudaMemcpyDeviceToHost));
     }

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for librwgpu (sm_100a).
+// common.cuh -- shared host/device helpers for librwgpu (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -26,6 +26,10 @@ const char* last_error_cstr();
     if (_e != cudaSuccess)                                                                 \
       return ::rw::fail(RW_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
   } while (0)
+
+// streaming multiprocessors of the H100 SXM; grid-stride kernels cap their grids at RW_SMS x 8 blocks of
+// 256 threads (2048 resident threads per SM)
+#define RW_SMS 132
 
 int type_width(int t);
 bool type_is_float(int t);

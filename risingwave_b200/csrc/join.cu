@@ -1,4 +1,4 @@
-// join.cu -- streaming two-sided incremental HashJoin on sm_100a.
+// join.cu -- streaming two-sided incremental HashJoin on sm_90a.
 //
 // Replaces (reference, Rust):
 //   HashJoinExecutor::eq_join_oneside      src/stream/src/executor/hash_join.rs:925-1062
@@ -17,8 +17,7 @@
 //                  Key64 + 48 B record = 64 B: a probe of a key with one row (bid -> auction) is ONE
 //                  64-byte random access that returns key, count and the row; an insert into a
 //                  fresh key is one 64-byte read-modify-write.  (Random 64 B transactions are what
-//                  bounds this workload: measured 42 G random loads/s, 22 G random RMW/s on B200,
-//                  profiles/r1_ubench_atomics.txt.)
+//                  bounds this workload; tools/ubench_atomics.cu measures their rate.)
 //   overflow store: further rows of a key go to an append-only array of records chained through
 //                  `link` from the bucket's head.
 // Two execution paths:
@@ -54,7 +53,7 @@ namespace rw {
 //   bits 31..32  state of the inline record: 0 = never used, 1 = live, 2 = dead (reusable)
 //   bits 33..63  live row count of the key (inline + overflow)
 // Every own-side mutation of a bucket is ONE compare-and-swap on W (or one 128-bit CAS on key|W
-// when the bucket is claimed): random atomics are the scarce resource (22 G/s on B200).
+// when the bucket is claimed): random atomics are the scarce resource.
 #define W_EMPTY 0x7fffffffull
 #define W_COUNT_ONE (1ull << 33)
 #define W_IL_LIVE (1ull << 31)
@@ -847,7 +846,7 @@ __global__ void __launch_bounds__(JF_BLOCK, 8) join_inner_fused_kernel(const Joi
 // Rows it cannot take (key == EMPTY sentinel, matched record with NULLs, keys with several rows)
 // fall through to the same helpers the generic kernel uses.
 #define W8_MAXC 8
-#define Q4_MAX_GRID (148 * 8)  // blocks of JF_BLOCK threads; one row-id pool per warp
+#define Q4_MAX_GRID (RW_SMS * 8)  // blocks of JF_BLOCK threads; one row-id pool per warp
 struct W8Plan {
   int n_u, n_m;            // columns of the update / matched side (all 8 bytes wide)
   int key_col;             // key column of the update side
@@ -1060,11 +1059,11 @@ __device__ __forceinline__ int64_t chunk_rows(const DevChunk& ch, JoinStatus* st
 }
 
 // ------------------------------------------------------------------ quad-cooperative Key64 kernel (<= 4 + 4 columns)
-// tools/ubench_bucket.cu (profiles/r1_ubench_bucket.txt): what a random bucket access costs is the
-// number of memory INSTRUCTIONS that touch the line, not its bytes -- one thread reading a 64-byte
-// bucket with 4 x LDG.128 takes 90 us per 2^20 rows, four lanes reading 16 bytes each in ONE
-// instruction take 25 us (the price of a single 16-byte load); a record written with three 16-byte
-// stores costs 89 us cold but ~17 us once the claiming CAS has pulled the line into L2.
+// tools/ubench_bucket.cu: what a random bucket access costs is the number of memory INSTRUCTIONS that
+// touch the line, not its bytes -- one thread reading a 64-byte bucket with 4 x LDG.128 costs several
+// times what four lanes reading 16 bytes each in ONE instruction cost (the price of a single 16-byte
+// load); a record written with three 16-byte stores is cheap once the claiming CAS has pulled the line
+// into L2.
 // So a row is owned by a QUAD of lanes and a warp works on 8 rows:
 //   lane q of the quad loads piece q of the other side's bucket   [key|W] [rec hdr] [col0,col1] [col2,col3]
 //   lanes 0,1 hold the update row's columns (0,1) / (2,3) and write them to the output,
@@ -1076,10 +1075,12 @@ __device__ __forceinline__ int64_t chunk_rows(const DevChunk& ch, JoinStatus* st
 // record, NULLs in the matched record) are finished by lane 0 with the generic helpers.
 // Output convention: positional, exactly as join_inner_w8p_kernel.
 struct U256 { uint64_t a, b, c, d; };
-// one 32-byte load (LDG.E.256, sm_100), L2 only
+// 32 bytes of one sector, L2 only: sm_90 has no 256-bit load, so two 16-byte loads issued back to back
+// (both in flight together; the second hits the sector the first one requested)
 __device__ __forceinline__ U256 ld256_cg(const void* ptr) {
   U256 v;
-  asm volatile("ld.global.cg.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(v.a), "=l"(v.b), "=l"(v.c), "=l"(v.d) : "l"(ptr));
+  asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
+               : "=l"(v.a), "=l"(v.b), "=l"(v.c), "=l"(v.d) : "l"(ptr));
   return v;
 }
 __device__ __forceinline__ uint64_t shfl64m(unsigned mask, uint64_t v, int src) {
@@ -1095,7 +1096,7 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) join_inner_q4_kernel(const Joi
   const int lane = lane_id(), q = lane & 3, qlead = lane & ~3;
   // Overflow row ids come from a per-warp pool that persists across launches: one atomicAdd on the
   // shared counter hands a warp `pool_chunk` ids.  (One atomicAdd per 8 rows on that single address
-  // was measured at +0.3 ms per 2^20 rows -- same-address atomics serialise in one L2 slice.)
+  // was slower -- same-address atomics serialise in one L2 slice.)
   const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   uint32_t pool_next = 0, pool_end = 0;
   if (!PROBE_ONLY) {
@@ -1129,7 +1130,7 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) join_inner_q4_kernel(const Joi
   cas_empty.y = W_EMPTY;
   cas_want.y = (W_EMPTY | W_IL_LIVE) + W_COUNT_ONE;
   // All shuffles use the full-warp mask and sit in warp-uniform control flow: a shuffle with a
-  // per-quad mask splits the warp into eight separately issued groups (measured: 2.8x slower).
+  // per-quad mask splits the warp into eight separately issued groups.
   // Software pipeline: the (sequential) column loads of the warp's NEXT group are issued right after
   // the random accesses of the current one, so they are out of the dependent chain
   // ops -> key -> bucket / CAS -> chain CAS that bounds this latency-bound kernel.
@@ -1714,8 +1715,8 @@ using namespace rw;
 struct SegLog {
   std::vector<DevBuf> segs;
   DevBuf table;  // U_MAX_SEGS device pointers
-  // ONE segment is allocated ahead of need by a helper thread (a 200 MB cudaMalloc takes 1.5-2 ms on the GPU boxes:
-  // on the push path the GPU would idle for ten steps' worth of time)
+  // ONE segment is allocated ahead of need by a helper thread (a 200 MB cudaMalloc takes milliseconds: on the push
+  // path the GPU would idle for several steps' worth of time)
   std::thread worker;
   std::mutex mu;
   DevBuf spare;
@@ -1899,7 +1900,7 @@ struct rwgpu_join {
 
 static int jgrid(int64_t n, int block) {
   int64_t g = (n + block - 1) / block;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(g, 148 * 8));
+  return (int)std::max<int64_t>(1, std::min<int64_t>(g, RW_SMS * 8));
 }
 
 static JoinSideDev side_dev(const rwgpu_join* h, int S) {
@@ -2383,8 +2384,17 @@ static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, u
   {
     JoinSideHost& own = h->side[pd.S];
     const uint64_t n = (uint64_t)pd.ch.n, slack = (uint64_t)pd.grid * 8 * pd.pool_chunk;
-    own.n_rows = hs.log_next[pd.S] + (own.n_rows - (pd.ids_before + n + slack));
-    h->uni_keys = hs.n_keys[0] + (h->uni_keys - (pd.keys_before + n));
+    const uint64_t rows_now = hs.log_next[pd.S] + (own.n_rows - (pd.ids_before + n + slack));
+    const uint64_t keys_now = hs.n_keys[0] + (h->uni_keys - (pd.keys_before + n));
+    // the pushes still outstanding (already popped off: h->pending holds only later ones) took their "before" values
+    // from the bounds replaced here: shift them alike, or their own collect subtracts this correction a second time
+    // and the unsigned bounds wrap
+    for (int i = 0; i < h->n_pending; i++) {
+      h->pending[i].ids_before += rows_now - own.n_rows;
+      h->pending[i].keys_before += keys_now - h->uni_keys;
+    }
+    own.n_rows = rows_now;
+    h->uni_keys = keys_now;
     h->uni_keys_exact = hs.n_keys[0];
   }
   hs.err = err;
@@ -2480,8 +2490,8 @@ static int join_push_dev(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream
       const int grid = q4 ? q4_grid : jgrid(n, JF_BLOCK);
       auto launch = [&](bool probe_only, uint32_t store_base) {
         if (q4) {
-          // 4 blocks of 256 threads per SM (64 registers).  Measured per 2^20 rows: 3 blocks/SM 0.262 ms, 4: 0.227,
-          // 5: 0.267, 6: 0.300, 8: 0.329 -- the kernel is bound by random DRAM transactions, not by occupancy.
+          // 4 blocks of 256 threads per SM (64 registers): the kernel is bound by random DRAM transactions, not by
+          // occupancy, and more resident blocks do not make it faster.
           if (probe_only)
             join_inner_q4_kernel<true, 4><<<grid, JF_BLOCK, 0, st>>>(pd, h->w8[S], S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h),
                                                                       ds, store_base, seq_base, out_base, pool_chunk);
@@ -2538,7 +2548,7 @@ static int join_push_dev(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream
       h->out_rows_cumulative = true;
       h->call_vis_stale = true;
       const int64_t tiles = (n + JF_BLOCK * JF_R - 1) / (JF_BLOCK * JF_R);
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, 148 * 8));
+      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(tiles, RW_SMS * 8));
       h->prof.begin(st);
       join_inner_fused_kernel<false><<<grid, JF_BLOCK, 0, st>>>(pd, S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h), ds,
                                                                   (uint32_t)own.n_rows, seq_base);
@@ -3142,7 +3152,7 @@ int32_t rwgpu_join_push(rwgpu_join* h, int32_t side, const rw_chunk* c, rwgpu_ou
       RW_CUDA(cudaEventCreateWithFlags(&h->ev_main[i], cudaEventDisableTiming));
     }
   }
-  // each sub-batch costs one status read-back (~40 us): keep them >= 32K rows
+  // each sub-batch costs one status read-back: keep them >= 32K rows
   const int J = n >= (1 << 19) ? 8 : (n >= (1 << 17) ? 4 : (n >= (1 << 16) ? 2 : 1));
   int64_t sub = (n + J - 1) / J;
   sub = (sub + 63) / 64 * 64;
@@ -3503,6 +3513,10 @@ int32_t rwgpu_join_collect_out(rwgpu_join* h, rwgpu_out** out) {
   if (rc != RW_OK) return bail(rc);
   rc = join_post_process(h, total, &nullm, pd.st);
   if (rc != RW_OK) return bail(rc);
+  // the copies below run on the copy-out stream: order them behind the post-process, which may rewrite ops / visibility
+  // on the main stream (the push itself was collected, so its event can be recorded again)
+  RW_CUDA(cudaEventRecord(h->pend_ev[pd.set], pd.st));
+  RW_CUDA(cudaStreamWaitEvent(sd, h->pend_ev[pd.set], 0));
   const int64_t n = hp.n;
   // what the launch already copied is good unless the emission was redone into re-allocated buffers
   bool pre_ok = h->os().out_ops.as<uint8_t>() == ops_before && total >= n;

@@ -1,6 +1,6 @@
 // join_uni.cuh -- ONE hash table for both sides of a Key64 inner join (included by join.cu).
 //
-// Round-1 measurement (profiles/README.md): the two-table inner kernel is bound by the NUMBER of random
+// The two-table inner kernel (join.cu) is bound by the NUMBER of random
 // 64-byte DRAM transactions per row -- probe line of the other side, own-side line read by the claiming
 // CAS, own-side write-back, and each 128-byte bucket-pair fetch counted twice.  Here a join key owns ONE
 // 64-byte bucket that carries the state of BOTH sides, so a row's probe and its own-side insert touch the
@@ -34,7 +34,7 @@ namespace rw {
 
 // A side's log is a list of fixed-size SEGMENTS (2^22 records = 192 MiB each) reached through a small device table of
 // segment pointers: growing the log allocates one more segment and appends its pointer -- no copy of the existing
-// hundreds of megabytes in the middle of the stream (round 1: allocate + copy + free, 0.3-0.7 ms per event), no
+// hundreds of megabytes in the middle of the stream (as allocate + copy + free of the whole store would), no
 // contiguous virtual range.  Record id -> segment id >> 22, offset (id & 2^22-1) * 48.
 #define U_SEG_SHIFT 22
 #define U_SEG_RECS (1u << U_SEG_SHIFT)
@@ -131,47 +131,76 @@ __device__ __forceinline__ void uni_emit(const JoinOutDev& o, const W8Plan& w, J
   if (nullbits) atomicOr(&st->null_mask, nullbits);
 }
 
-// emit the `cnt` matches of chunk row r found in bucket b: the first at the positional row `pos`, the others at
-// xpos, xpos + 1, ...  (S = side of the chunk row)
+// emit the `cnt` matches of chunk row r found in bucket b: one at the positional row `pos`, the others at
+// xpos, xpos + 1, ...  (S = side of the chunk row).  The positional row gets the live match that ARRIVED LAST (largest
+// arrival number): the positional rows of a U- / U+ pair are adjacent, so that match's pair is the one the no-op pass
+// hides, and it must not depend on the order in which concurrent inserts linked the chain.  Rows are pushed at the chain's
+// head, so the walk usually meets the last arrival first; when concurrent inserts of one chunk linked out of order, the
+// two rows are swapped at the end (matches are kept as references and re-read for the swap: holding their columns
+// doubled the kernels' registers).
 __device__ __forceinline__ void uni_emit_matches(const UniDev& t, const W8Plan& w, int S, const DevChunk& ch, int64_t r, uint8_t oop, int64_t b,
                                                  uint32_t cnt, const JoinOutDev& o, JoinStatus* st, int64_t pos, int64_t xpos) {
-  uint32_t left = cnt;
-  bool first = true;
-  auto place = [&]() -> int64_t {
-    if (first) { first = false; return pos; }
-    o.vis[xpos] = 1;
-    return xpos++;
+  const uint64_t SEQ56 = (1ull << 56) - 1;
+  const uint32_t IL = 0xffffffffu;  // reference to the bucket's inline record (log ids are < 2^31)
+  const int mside = S != t.is ? t.is : 1 - t.is;
+  // one match: columns + null mask of the inline record or of log record m
+  auto load = [&](uint32_t m, uint64_t* mc, uint32_t* nm) {
+    const uint8_t* base = m == IL ? ub(t, b) + 32 : (const uint8_t*)urec(t, mside, m) + 16;
+    const ulonglong2 c01 = __ldcg((const ulonglong2*)base), c23 = __ldcg((const ulonglong2*)base + 1);
+    mc[0] = c01.x; mc[1] = c01.y; mc[2] = c23.x; mc[3] = c23.y;
+    *nm = m == IL ? (uint32_t)(__ldcg(ub_IH(t, b)) & 0xffull) : __ldcg(&urec(t, mside, m)->nullmask);
+  };
+  uint32_t left = cnt, pos_ref = U_NIL, best_ref = U_NIL;
+  uint64_t best_seq = 0;
+  int64_t best_at = pos;
+  auto put = [&](uint32_t m, uint64_t seq) {
+    int64_t at = pos;
+    if (pos_ref == U_NIL) {
+      pos_ref = m;
+      best_seq = seq;
+    } else {
+      at = xpos++;
+      o.vis[at] = 1;
+      if (seq > best_seq) { best_seq = seq; best_ref = m; best_at = at; }
+    }
+    uint64_t mc[4];
+    uint32_t nm;
+    load(m, mc, &nm);
+    uni_emit(o, w, st, at, oop, ch, r, mc, nm);
   };
   uint32_t m;
-  int mside;
   if (S != t.is) {  // matches are the inline side's rows: the bucket's inline record, then the WI chain
     const unsigned long long WI = __ldcg(ub_WI(t, b));
     if (W_istate(WI) == 1u) {
-      const unsigned long long ih = __ldcg(ub_IH(t, b));
-      uint64_t mc[4];
-      const ulonglong2 c01 = __ldcg((const ulonglong2*)(ub(t, b) + 32)), c23 = __ldcg((const ulonglong2*)(ub(t, b) + 48));
-      mc[0] = c01.x; mc[1] = c01.y; mc[2] = c23.x; mc[3] = c23.y;
-      uni_emit(o, w, st, place(), oop, ch, r, mc, (uint32_t)(ih & 0xffull));
-      if (--left == 0) return;
+      put(IL, (__ldcg(ub_IH(t, b)) >> 8) & SEQ56);
+      left--;
     }
     m = W_head(WI);
-    mside = t.is;
   } else {
     m = __ldcg(ub_chead(t, b));
-    mside = 1 - t.is;
   }
   while (m != U_NIL && left) {
-    const UniRec* rec = urec(t, mside, m);
-    const ulonglong2 h0 = __ldcg((const ulonglong2*)rec);  // link | nullmask, seq
+    const ulonglong2 h0 = __ldcg((const ulonglong2*)urec(t, mside, m));  // link | nullmask, seq
     const uint32_t lk = (uint32_t)h0.x;
     if (!(lk & J_DEAD)) {
-      uint64_t mc[4];
-      const ulonglong2 c01 = __ldcg((const ulonglong2*)rec + 1), c23 = __ldcg((const ulonglong2*)rec + 2);
-      mc[0] = c01.x; mc[1] = c01.y; mc[2] = c23.x; mc[3] = c23.y;
-      uni_emit(o, w, st, place(), oop, ch, r, mc, (uint32_t)(h0.x >> 32));
+      put(m, h0.y & SEQ56);
       left--;
     }
     m = lk & 0x7fffffffu;
+  }
+  if (best_at != pos) {  // the last arrival goes to the positional row, the row that was there takes its place
+    uint64_t mc[4];
+    uint32_t pos_nm, best_nm;
+    load(pos_ref, mc, &pos_nm);
+    load(best_ref, mc, &best_nm);
+    for (int c = 0; c < 4; c++) {  // (uni_emit only clears valid bytes: set back the ones the first emission cleared)
+      if (c >= w.n_m || w.m_out[c] < 0) continue;
+      if ((pos_nm >> c) & 1u) o.valid[w.m_out[c]][pos] = 1;
+      if ((best_nm >> c) & 1u) o.valid[w.m_out[c]][best_at] = 1;
+    }
+    uni_emit(o, w, st, pos, oop, ch, r, mc, best_nm);
+    load(pos_ref, mc, &pos_nm);
+    uni_emit(o, w, st, best_at, oop, ch, r, mc, pos_nm);
   }
 }
 
@@ -280,7 +309,7 @@ __device__ __forceinline__ ulonglong2 ld128_cg(const void* ptr) { return __ldcg(
 // ------------------------------------------------------------------ quad-cooperative kernel (plain chunks)
 // A row is owned by a QUAD of lanes, a warp works on 8 rows per iteration.  Lane q loads 16 bytes of the key's
 // bucket in ONE instruction per quad (the cost of a random bucket access is the number of memory instructions
-// that reach the line, profiles/r1_ubench_bucket.txt):
+// that reach the line, tools/ubench_bucket.cu):
 //     lane 0: key | WI      lane 1: IH | WC      lane 2: inline columns 0,1      lane 3: inline columns 2,3
 // lanes 0,1 hold the update row's columns (0,1) / (2,3) and write them to the output; lanes 2,3 write the
 // matched columns they loaded themselves -- no shuffle moves payload.  Lane 0 then does the own-side state
@@ -784,7 +813,7 @@ __device__ __forceinline__ void uni_delete_body(const JoinPlanDev* __restrict__ 
 // later in the chunk may target it).  When a batch has both (n_defer bit 1 and deletes), the deletes of sentinel-key
 // rows are left to the LAST block, which runs them after every other block has finished: no block ever waits for
 // another one, so the kernel needs no co-residency and no cooperative launch.
-// (r2b: separate deferred and delete launches ~9 us each; r2d: as a cooperative launch 37 us per step; plain: 15 us.)
+// (Separate deferred and delete launches, or one cooperative launch, each cost more per step than this plain one.)
 template <bool PROBE_ONLY>
 __global__ void __launch_bounds__(256) uni_tail_kernel(const JoinPlanDev* __restrict__ p, W8Plan w, int S, DevChunk ch, UniDev t, JoinOutDev o, UniWork wk,
                                                        JoinStatus* st, uint64_t seq_base, int64_t out_base, JoinStatus* status_host,

@@ -1,4 +1,4 @@
-// shuffle.cu -- the hash-shuffle (vnode) path on sm_100a.
+// shuffle.cu -- the hash-shuffle (vnode) path on sm_90a.
 //
 // Replaces (reference, Rust):
 //   VirtualNode::compute_chunk              src/common/src/hash/consistent_hash/vnode.rs:151-182
@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(PART_BLOCK) part_hist_kernel(DevChunk ch, Vnod
 
 // pass 2: one block; per destination exclusive scan over blocks -> block offsets; totals + region starts.
 // One WARP per destination scans the per-block counts 32 at a time (shuffle scan, the chunk loads do
-// not depend on each other); a serial loop over 512 blocks per thread cost ~100 us of a 1M-row batch.
+// not depend on each other); a serial loop over 512 blocks per thread was far slower.
 #define PART_SCAN_THREADS 1024
 __global__ void __launch_bounds__(PART_SCAN_THREADS) part_scan_kernel(uint32_t* block_hist, int n_blocks, int n_dest, int64_t* counts,
                                                                        int64_t* offsets) {
@@ -496,7 +496,7 @@ __device__ __forceinline__ void flat_barrier(const PeerBases& flags, int n, int 
 
 // grid-wide barrier of a PLAIN launch whose grid is sized to be resident (flat_exchange_kernel): `bar` counts arrivals
 // and is never reset inside a launch -- barrier number k (1, 2, ...) waits for k * gridDim.x.  A cooperative launch
-// (grid.sync()) cost ~20 us more per launch on the join's tail kernel and cannot start before EVERY block fits; this
+// (grid.sync()) costs more per launch and cannot start before EVERY block fits; this
 // one starts with the blocks that fit and the rest follow as a neighbour kernel drains.
 __device__ __forceinline__ void soft_grid_sync(unsigned int* bar, unsigned int k) {
   __syncthreads();
@@ -513,7 +513,7 @@ __device__ __forceinline__ void soft_grid_sync(unsigned int* bar, unsigned int k
 // STAGED (every column 8 bytes wide): a tile's rows are first partitioned into SHARED MEMORY (stable, destination by
 // destination) and then written out with consecutive threads storing consecutive rows of a destination's segment -- a
 // warp's store instruction covers 256 contiguous bytes of ONE peer instead of 8-byte pieces scattered over all of them
-// (r2 4-GPU run: the per-row peer stores sustained ~80 GB/s of NVLink's 900).  Otherwise rows go out one by one.
+// (per-row peer stores reach a small fraction of NVLink's bandwidth).  Otherwise rows go out one by one.
 #define FLAT_TILE 1024
 template <bool STAGED>
 __global__ void __launch_bounds__(PART_BLOCK) flat_exchange_kernel(DevChunk ch, VnodePlan p, const int32_t* vnode_to_dest, int n_dest, int my_rank,
@@ -708,7 +708,7 @@ static int make_vnode_plan(const rw_chunk* c, const int32_t* keys, int n_keys, i
 
 static int grid_rows(int64_t n, int block) {
   int64_t g = (n + block - 1) / block;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(g, 148 * 8));
+  return (int)std::max<int64_t>(1, std::min<int64_t>(g, RW_SMS * 8));
 }
 
 // upload a HOST rw_chunk into one temporary device allocation
@@ -949,7 +949,7 @@ int32_t rwgpu_shuffle_unpack_device(const void* recv_base, int32_t n_src, const 
   PartOut o;
   memset(&o, 0, sizeof(o));
   for (int k = 0; k < n_cols; k++) o.col[k] = out_cols[k];
-  p2p_unpack_kernel<<<148 * 4, 256, 0, (cudaStream_t)cuda_stream>>>((const uint8_t*)recv_base, n_src, L, out_ops, o, total);
+  p2p_unpack_kernel<<<RW_SMS * 4, 256, 0, (cudaStream_t)cuda_stream>>>((const uint8_t*)recv_base, n_src, L, out_ops, o, total);
   RW_CUDA(cudaGetLastError());
   return RW_OK;
 }
@@ -1008,7 +1008,7 @@ int32_t rwgpu_shuffle_exchange_flat_device(const rw_chunk* c, const int32_t* key
     } else {
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, flat_exchange_kernel<false>, PART_BLOCK, 0);
     }
-    // three blocks per SM: measured best next to the join's kernel at N=2 (profiles/README.md: 296 / 444 / 888 blocks)
+    // at most three blocks per SM, so that the join's kernel keeps SM slots beside the exchange
     cores = std::max(1, sms * std::max(1, std::min(per_sm, 3)));
   }
   int grid = std::min(n_vblocks, cores);
@@ -1023,7 +1023,7 @@ int32_t rwgpu_shuffle_exchange_flat_device(const rw_chunk* c, const int32_t* key
   unsigned int* bar = (unsigned int*)(scratch + dest_bytes + 2 * hist_bytes);
   RW_CUDA(cudaMemsetAsync(bar, 0, 4, st));
   // RWGPU_EXCHANGE_COOP=1: cooperative launch (grid.sync()) instead of the software barriers -- the whole grid starts at
-  // once, which on the 2-GPU runs let the join's kernel fill in around it (profiles/README.md, multi-GPU table)
+  // once, and the join's kernel fills in around it
   static const int coop = getenv("RWGPU_EXCHANGE_COOP") ? atoi(getenv("RWGPU_EXCHANGE_COOP")) : 0;
   int coop_arg = coop;
   unsigned long long ep = epoch;

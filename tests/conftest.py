@@ -10,7 +10,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a machine with an H100)")
 
 
 def _oracle_lib_path():

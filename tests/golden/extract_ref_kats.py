@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """Extract the reference's golden vectors for the HashJoin / HashAgg / dispatch path into JSON.
 
-Run in the BUILD container only (it reads /root/reference, which does not exist on the GPU box):
+Reads a checkout of risingwavelabs/risingwave; the tests only read the committed JSON:
 
-    python tests/golden/extract_ref_kats.py
+    python tests/golden/extract_ref_kats.py <risingwave checkout> [output directory, default: this directory]
 
 Outputs (committed):
     tests/golden/hash_join_kats.json   <- src/stream/src/executor/hash_join.rs  #[tokio::test]s
@@ -22,8 +22,8 @@ import os
 import re
 import sys
 
-REF = "/root/reference"
-OUT = os.path.dirname(os.path.abspath(__file__))
+REF = sys.argv[1] if len(sys.argv) > 1 else ""
+OUT = sys.argv[2] if len(sys.argv) > 2 else os.path.dirname(os.path.abspath(__file__))
 
 
 def clean_pretty(lit: str) -> str:
@@ -302,7 +302,7 @@ def extract_nexmark_q4():
 
 def main():
     if not os.path.isdir(REF):
-        sys.exit("reference not mounted; fixtures are committed, nothing to do")
+        sys.exit("usage: extract_ref_kats.py <risingwave checkout> [output directory]")
     hj = extract_hash_join()
     json.dump(hj, open(os.path.join(OUT, "hash_join_kats.json"), "w"), indent=1)
     ha = extract_hash_agg()

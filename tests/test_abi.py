@@ -30,7 +30,7 @@ def test_type_width_and_version():
     for t, w in abi.TYPE_WIDTH.items():
         assert lib.rwgpu_type_width(t) == w
     lib.rwgpu_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in lib.rwgpu_version()
+    assert b"sm_90a" in lib.rwgpu_version()
 
 
 def test_struct_sizes_match_header():

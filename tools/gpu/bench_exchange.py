@@ -19,7 +19,7 @@ stream = torch.cuda.Stream()
 for world in (1, 2, 8):  # world > 1: the destinations are virtual (all buffers on this device); only rank 0's kernel runs -> world 1 for barriers
     pass
 total, ops_off, col_off = device.flat_layout(T4, N)
-for max_blocks in (0, 296, 148):
+for max_blocks in (0, 2 * 132, 132):  # default (resident grid), two and one blocks per H100 SM
     buf = torch.zeros(total, dtype=torch.uint8, device="cuda")
     flags = torch.zeros(1024, dtype=torch.uint8, device="cuda")
     counts = torch.zeros(1, dtype=torch.int64, device="cuda")

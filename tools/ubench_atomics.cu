@@ -1,5 +1,5 @@
-// ubench_atomics.cu -- random-access load / atomic throughput on a table much larger than L2 (B200).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build/ubench_atomics tools/ubench_atomics.cu
+// ubench_atomics.cu -- random-access load / atomic throughput on a table much larger than L2 (H100).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/ubench_atomics tools/ubench_atomics.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -49,9 +49,9 @@ __global__ void k(ulonglong2* tab, uint64_t mask, uint64_t n, uint64_t seed, uns
 
 template <int MODE> void run(const char* name, ulonglong2* tab, uint64_t slots, uint64_t n, unsigned long long* sink) {
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-  k<MODE><<<148 * 8, 256>>>(tab, slots - 1, n, 1, sink);
+  k<MODE><<<132 * 8, 256>>>(tab, slots - 1, n, 1, sink);
   cudaEventRecord(a);
-  for (int it = 0; it < 3; it++) k<MODE><<<148 * 8, 256>>>(tab, slots - 1, n, 77 + it, sink);
+  for (int it = 0; it < 3; it++) k<MODE><<<132 * 8, 256>>>(tab, slots - 1, n, 77 + it, sink);
   cudaEventRecord(b); cudaEventSynchronize(b);
   float ms; cudaEventElapsedTime(&ms, a, b); ms /= 3;
   printf("%-34s table %5.0f MB  %7.2f G ops/s  (%.3f ms for %llu ops)\n", name, slots * 16.0 / 1e6, n / ms / 1e6, ms, (unsigned long long)n);

@@ -1,7 +1,8 @@
 // ubench_bucket.cu -- how should one thread (or a few lanes) touch a random 64-byte bucket in HBM?
 // ubench_probe showed 4 x LDG.128 of one bucket costs 3.5x one LDG.128.  This measures the alternatives:
-// 256-bit loads/stores (LDG.E.256, sm_100), lane-cooperative access, and the insert-side sequences.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build/ubench_bucket tools/ubench_bucket.cu
+// 32-byte accesses (sm_90 has no 256-bit load: two 16-byte instructions on one sector), lane-cooperative access,
+// and the insert-side sequences.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/ubench_bucket tools/ubench_bucket.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -9,11 +10,13 @@ __device__ __forceinline__ uint64_t mix64(uint64_t x) { x ^= x >> 33; x *= 0xff5
 struct U4 { uint64_t a, b, c, d; };
 __device__ __forceinline__ U4 ld256(const void* p) {
   U4 v;
-  asm volatile("ld.global.cg.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(v.a), "=l"(v.b), "=l"(v.c), "=l"(v.d) : "l"(p));
+  asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
+               : "=l"(v.a), "=l"(v.b), "=l"(v.c), "=l"(v.d) : "l"(p));
   return v;
 }
 __device__ __forceinline__ void st256(void* p, U4 v) {
-  asm volatile("st.global.cg.v4.u64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(v.a), "l"(v.b), "l"(v.c), "l"(v.d) : "memory");
+  asm volatile("st.global.cg.v2.u64 [%0], {%1,%2};\n\tst.global.cg.v2.u64 [%0+16], {%3,%4};"
+               ::"l"(p), "l"(v.a), "l"(v.b), "l"(v.c), "l"(v.d) : "memory");
 }
 __device__ __forceinline__ bool cas128(void* addr, ulonglong2 expect, ulonglong2 desired, ulonglong2* found) {
   asm volatile(
@@ -151,7 +154,7 @@ int main() {
   uint8_t *tab, *tab2; cudaMalloc(&tab, buckets * 64); cudaMemset(tab, 1, buckets * 64);
   cudaMalloc(&tab2, buckets * 64); cudaMemset(tab2, 1, buckets * 64);
   const int64_t n = 1 << 22;
-  const int grid = 148 * 16;
+  const int grid = 132 * 16;
   run<L_16>("L  1 x 16B load", grid, tab, tab2, buckets, n, sink);
   run<L_4x16>("L  4 x 16B loads (current probe)", grid, tab, tab2, buckets, n, sink);
   run<L_PF_4x16>("L  prefetch.L2 + 4 x 16B loads", grid, tab, tab2, buckets, n, sink);

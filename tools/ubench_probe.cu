@@ -1,5 +1,5 @@
 // ubench_probe.cu -- build the join probe up from the raw random-load baseline to find what costs time.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build/ubench_probe tools/ubench_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/ubench_probe tools/ubench_probe.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -56,7 +56,7 @@ int main() {
     for (int64_t i = 0; i < n; i++) { uint64_t x = i * 0x9E3779B97F4A7C15ull; x ^= x >> 31; h[i] = x; }
     cudaMemcpy((void*)cs.c[0], h, n * 8, cudaMemcpyHostToDevice); free(h);
   }
-  for (int grid : {148 * 8, 148 * 16, (int)(n / 256)}) {
+  for (int grid : {132 * 8, 132 * 16, (int)(n / 256)}) {
     run<0>("V0 random 16B load from 64B bucket", grid, tab, buckets, n, cs, sink);
     run<1>("V1 + whole 64B bucket (4 x 16B)", grid, tab, buckets, n, cs, sink);
     run<2>("V2 + key from column", grid, tab, buckets, n, cs, sink);

@@ -6,7 +6,7 @@
 //   B  heads in a separate dense 4-byte array indexed by bucket number (64 MB: L2-resident?), atomicExch
 //   B' same with L2 evict_last on the heads and evict_first on every stream / the bucket loads
 //   C  probe + emit only (read-only floor)
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build/ubench_unified tools/ubench_unified.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/ubench_unified tools/ubench_unified.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -180,7 +180,7 @@ int main(int argc, char** argv) {
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, 0);
   printf("L2 %d MB, persistingL2CacheMaxSize %d MB, accessPolicyMaxWindowSize %d MB\n", prop.l2CacheSize >> 20, prop.persistingL2CacheMaxSize >> 20,
          prop.accessPolicyMaxWindowSize >> 20);
-  for (int grid : {148 * 4, 148 * 8}) {
+  for (int grid : {132 * 4, 132 * 8}) {
     run<V_C, 4>("C  probe + emit only (no own-side insert)", grid, a, nb, n, sink, false, st);
     run<V_A, 4>("A  unified bucket: CAS64 on W_L in the probed line + log append", grid, a, nb, n, sink, false, st);
     run<V_A_NOREC, 4>("A- same without the log append", grid, a, nb, n, sink, false, st);
@@ -188,8 +188,8 @@ int main(int argc, char** argv) {
     run<V_BH, 4>("B' same, evict_last on heads / evict_first on streams+buckets", grid, a, nb, n, sink, false, st);
     run<V_B_NOOUT, 4>("B- heads variant without output stores", grid, a, nb, n, sink, false, st);
   }
-  run<V_A, 8>("A  (8 blocks/SM, 32 regs)", 148 * 8, a, nb, n, sink, false, st);
-  run<V_B, 8>("B  (8 blocks/SM, 32 regs)", 148 * 8, a, nb, n, sink, false, st);
+  run<V_A, 8>("A  (8 blocks/SM, 32 regs)", 132 * 8, a, nb, n, sink, false, st);
+  run<V_B, 8>("B  (8 blocks/SM, 32 regs)", 132 * 8, a, nb, n, sink, false, st);
   // persisting-L2 window on the heads array
   size_t want = (size_t)buckets * 4;
   if (prop.persistingL2CacheMaxSize > 0) {
@@ -202,9 +202,9 @@ int main(int argc, char** argv) {
     attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
     cudaError_t e = cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &attr);
     printf("access policy window: %s\n", cudaGetErrorString(e));
-    run<V_B, 4>("B  heads[] with persisting access-policy window", 148 * 4, a, nb, n, sink, true, st);
-    run<V_B, 4>("B  heads[] with persisting access-policy window", 148 * 8, a, nb, n, sink, true, st);
-    run<V_A, 4>("A  (window set on heads: control)", 148 * 4, a, nb, n, sink, true, st);
+    run<V_B, 4>("B  heads[] with persisting access-policy window", 132 * 4, a, nb, n, sink, true, st);
+    run<V_B, 4>("B  heads[] with persisting access-policy window", 132 * 8, a, nb, n, sink, true, st);
+    run<V_A, 4>("A  (window set on heads: control)", 132 * 4, a, nb, n, sink, true, st);
   }
   return 0;
 }
