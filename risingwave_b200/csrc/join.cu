@@ -2229,8 +2229,7 @@ static int uni_launch_main(rwgpu_join* h, const JoinPending& pd, bool probe_only
     po.capacity = od.capacity;
     // resident blocks per SM (registers per thread): 4 (64) by default; RWGPU_UNI_MINB=3 / 5 / 6 for tuning runs
     static const int minb = getenv("RWGPU_UNI_MINB") ? atoi(getenv("RWGPU_UNI_MINB")) : 4;
-    static const uint32_t kflags = getenv("RWGPU_UNI_FLAGS") ? (uint32_t)atoi(getenv("RWGPU_UNI_FLAGS")) : 0u;  // bit 0: L2 prefetch of the next bucket (key column two groups ahead), bit 1: deferred link store
-#define UNI_LAUNCH(PO, IS, MB) uni_hot_kernel<PO, IS, MB><<<pd.grid, JF_BLOCK, 0, pd.st>>>(pc, t.buckets, t.cap, own, po, wk, ds, pd.seq_base, pd.out_base, pd.pool_chunk, kflags)
+#define UNI_LAUNCH(PO, IS, MB) uni_hot_kernel<PO, IS, MB><<<pd.grid, JF_BLOCK, 0, pd.st>>>(pc, t.buckets, t.cap, own, po, wk, ds, pd.seq_base, pd.out_base, pd.pool_chunk)
     if (probe_only) {
       if (is_row) UNI_LAUNCH(true, true, 4); else UNI_LAUNCH(true, false, 4);
     } else if (is_row) {
@@ -2240,11 +2239,7 @@ static int uni_launch_main(rwgpu_join* h, const JoinPending& pd, bool probe_only
         case 3: UNI_LAUNCH(false, false, 3); break;
         case 5: UNI_LAUNCH(false, false, 5); break;
         case 6: UNI_LAUNCH(false, false, 6); break;
-        default:
-          if (kflags & 2u) uni_hot_kernel<false, false, 4, true><<<pd.grid, JF_BLOCK, 0, pd.st>>>(pc, t.buckets, t.cap, own, po, wk, ds, pd.seq_base, pd.out_base,
-                                                                                                pd.pool_chunk, kflags);
-          else UNI_LAUNCH(false, false, 4);
-          break;
+        default: UNI_LAUNCH(false, false, 4); break;
       }
     }
 #undef UNI_LAUNCH

@@ -17,11 +17,12 @@
 //                     a key goes to log[IS], chained from WI.head.
 //   chained side CS = the other one.  EVERY row is appended to log[CS] -- a sequential write: the 8 rows a
 //                     warp handles per iteration take consecutive ids from the warp's pool -- and pushed
-//                     on the key's chain with one atomicExch on WC.head (no CAS loop: hot keys serialise
-//                     in L2 only) + one RED on WC.count, both on the line the probe just loaded.
+//                     on the key's chain with one 64-bit atomicExch of WC = new head | loaded count + 1 (no CAS
+//                     loop: hot keys serialise in L2 only; a RED corrects the count when the key was contended,
+//                     uni_chain_push), on the line the probe just loaded.
 //   log record (48 B): u32 link | DEAD, u32 null mask, u64 seq, 4 x 8 B columns.
 //
-// A CS row (bid) therefore costs: one random 64 B read (key, WI, the matched auction row), two L2 atomics on
+// A CS row (bid) therefore costs: one random 64 B read (key, WI, the matched auction row), one L2 atomic on
 // that line (one 32/64 B write-back), 48 B appended to the log, 33 B read and 65 B written sequentially.
 // An IS row (auction) reads its bucket, walks the CS chain for matches, and claims the inline record.
 #pragma once
@@ -219,6 +220,21 @@ __device__ __forceinline__ uint32_t uni_alloc_one(const UniDev& t, int S, JoinSt
   return (uint32_t)id;
 }
 
+// Pushes log record `row` on a key's chained-side chain and returns the old head, the record's link.  WC = head | count << 32
+// is one aligned 8-byte word, so ONE 64-bit exchange writes both the new head and the count the caller expects, L + 1, where
+// L is the count the caller loaded with the bucket.  The exchange returns the count C it replaced; if another push or a
+// delete of the key moved the count since that load (C != L), C - L (mod 2^32) is added back.  Every other operation on the
+// count during a launch is an addition too (the correction, a delete's atomicSub), and in the order the atomics take effect
+// the exchange adds L + 1 - C: whatever the interleaving, the count after the launch is its old value plus the rows pushed
+// minus the rows deleted.  The head and the links come out as with an exchange of the head alone.  An uncontended push
+// costs one atomic; a push on a contended key costs two, as a separate head exchange and count increment always did.
+__device__ __forceinline__ uint32_t uni_chain_push(unsigned long long* wc, uint32_t row, uint32_t L) {
+  const unsigned long long old = atomicExch(wc, (unsigned long long)row | ((unsigned long long)(L + 1u) << 32));
+  const uint32_t C = (uint32_t)(old >> 32);
+  if (C != L) atomicAdd((uint32_t*)wc + 1, C - L);
+  return (uint32_t)old;
+}
+
 // own-side append of chunk row r to bucket b, by ONE thread (slow paths).  rid = a pre-allocated log id or U_NIL.
 __device__ __forceinline__ void uni_insert_row(const UniDev& t, int S, const DevChunk& ch, int n_cols, int64_t r, int64_t b, uint64_t seq,
                                                JoinStatus* st) {
@@ -242,8 +258,8 @@ __device__ __forceinline__ void uni_insert_row(const UniDev& t, int S, const Dev
   } else {
     const uint32_t rid = uni_alloc_one(t, S, st);
     if (rid == U_NIL) return;
-    const uint32_t old = atomicExch(ub_chead(t, b), rid);
-    atomicAdd(ub_ccount(t, b), 1u);
+    unsigned long long* wc = (unsigned long long*)ub_chead(t, b);
+    const uint32_t old = uni_chain_push(wc, rid, (uint32_t)(__ldcg(wc) >> 32));
     UniRec* rec = urec(t, S, rid);
     rec->link = old; rec->nullmask = nm; rec->seq = seq;
     rec->c[0] = c[0]; rec->c[1] = c[1]; rec->c[2] = c[2]; rec->c[3] = c[3];
@@ -353,13 +369,9 @@ struct UniWork {
   uint8_t* mask;     // [(n + 7) / 8], one bit per input row, every byte written by the hot kernel
 };
 
-// DL ("deferred link", chained-side rows only): the record's link word -- the old chain head the exchange returns -- is
-// stored by the exchanging lane at the top of the NEXT iteration, after that iteration's bucket load has been issued, so
-// the exchange's round trip overlaps the next bucket's instead of ending the iteration.
-template <bool PROBE_ONLY, bool IS_ROW, int MINB, bool DL = false>
+template <bool PROBE_ONLY, bool IS_ROW, int MINB>
 __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, uint8_t* buckets, uint64_t cap, UniOwn own, PlainOut o, UniWork wk,
-                                                                  JoinStatus* st, uint64_t seq_base, int64_t out_base, uint32_t pool_chunk,
-                                                                  uint32_t kflags) {
+                                                                  JoinStatus* st, uint64_t seq_base, int64_t out_base, uint32_t pool_chunk) {
   int64_t n_rows = ch.n;
   if (ch.n_dev) {
     const int64_t nd = *ch.n_dev;
@@ -379,55 +391,45 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
     pool_next = pl.x;
     pool_end = pl.y;
   }
-  const uint32_t pool_next0 = pool_next, pool_end0 = pool_end;
   int64_t xnext = 0, xend = 0;  // this warp's reservation in the extra-match area (offsets from xarea)
   const int64_t xarea = out_base + n_rows;
   const uint64_t mask = cap - 1;
   unsigned int new_keys = 0, n_del = 0;
-  bool any_match = false, any_hole = false, any_defer = false, any_sentinel = false;
+  // what this thread has seen, as bits of ONE register (separate booleans, each live across the loop, spilled)
+  enum : unsigned { SEEN_MATCH = 1u, SEEN_HOLE = 2u, SEEN_DEFER = 4u, SEEN_SENTINEL = 8u, SEEN_POOL = 16u };
+  unsigned seen = 0u;
   // (selected with ?: -- an index computed from the lane would put the parameter arrays in local memory)
   const unsigned long long* pa = (q & 1) ? ch.c[2] : ch.c[0];
   const unsigned long long* pb = (q & 1) ? ch.c[3] : ch.c[1];
   const unsigned long long* pk = ch.key;
-  unsigned long long* po0 = q == 0 ? o.ucol[0] : (q == 1 ? o.ucol[2] : (q == 2 ? o.mcol[0] : o.mcol[2]));
-  unsigned long long* po1 = q == 0 ? o.ucol[1] : (q == 1 ? o.ucol[3] : (q == 2 ? o.mcol[1] : o.mcol[3]));
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  // the two output columns lane q writes, s_po[q] and s_po[4 + q]: read from shared memory where a row is emitted (held in
+  // registers across the loop they were spilled to local memory)
+  __shared__ unsigned long long* s_po[8];
+  if (threadIdx.x < 8) {
+    const int c = threadIdx.x;
+    s_po[c] = c == 0 ? o.ucol[0] : c == 1 ? o.ucol[2] : c == 2 ? o.mcol[0] : c == 3 ? o.mcol[2]
+            : c == 4 ? o.ucol[1] : c == 5 ? o.ucol[3] : c == 6 ? o.mcol[1] : o.mcol[3];
+  }
+  __syncthreads();
+  const uint32_t nwarps = gridDim.x * (blockDim.x >> 5);
   const int64_t groups = (n_rows + 7) >> 3;
   const unsigned long long init_W = IS_ROW ? ((W_EMPTY | W_IL_LIVE) + W_COUNT_ONE) : W_EMPTY;
   // software pipeline: the sequential column loads of the warp's next group are issued right after the random
   // access of the current one
-  // (kflags bit 0) the KEY column runs two groups ahead: when group g's bucket load has been issued, the key of group
-  // g + 1 is already in a register (it was loaded during group g - 1), so its bucket line can be pulled into L2 at once
-  // -- a whole iteration before it is needed -- without waiting for anything.
   uint8_t n_op = 0;
-  unsigned long long n_key = J_EMPTY, n_va = 0ull, n_vb = 0ull, nn_key = J_EMPTY;
-  const bool pf = (kflags & 1u) != 0u;
+  unsigned long long n_key = J_EMPTY, n_va = 0ull, n_vb = 0ull;
 #define UNI_FETCH(G2)                                                             \
   do {                                                                            \
     const int64_t g2_ = (G2), r2_ = g2_ * 8 + (lane >> 2);                        \
     n_op = 0;                                                                     \
     if (g2_ < groups && r2_ < n_rows) {                                           \
       n_op = ch.ops[r2_];                                                         \
-      n_key = pf ? nn_key : __ldg(pk + r2_);                                      \
+      n_key = __ldg(pk + r2_);                                                    \
       if (pa) n_va = __ldg(pa + r2_);                                             \
       if (pb) n_vb = __ldg(pb + r2_);                                             \
-      if (pf) {                                                                   \
-        if (!(q & 1)) {                                                           \
-          const uint8_t* nb_ = buckets + uhome(n_key, mask) * 64 + 16 * q;        \
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(nb_));                    \
-        }                                                                         \
-        const int64_t r3_ = r2_ + nwarps * 8;                                     \
-        nn_key = (g2_ + nwarps < groups && r3_ < n_rows) ? __ldg(pk + r3_) : J_EMPTY; \
-      }                                                                           \
     }                                                                             \
   } while (0)
-  if (pf) {
-    const int64_t r0_ = warp_global * 8 + (lane >> 2);
-    if (warp_global < groups && r0_ < n_rows) nn_key = __ldg(pk + r0_);
-  }
   UNI_FETCH(warp_global);
-  unsigned long long pend_rec = 0ull;  // DL: record whose link word is still to be written (lane 0 of a quad)
-  uint32_t pend_link = 0u;
   for (int64_t g = warp_global; g < groups; g += nwarps) {
     const int64_t r = g * 8 + (lane >> 2);
     const bool in = r < n_rows;
@@ -449,7 +451,6 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
       if (first_iter) {
         UNI_FETCH(g + nwarps);
         first_iter = false;
-        if (DL && pend_rec) { *(unsigned long long*)pend_rec = (unsigned long long)pend_link; pend_rec = 0ull; }
       }
       const unsigned long long bkey = shfl64m(0xffffffffu, pv.x, qlead);
       const bool empty = need && bkey == J_EMPTY;
@@ -483,14 +484,14 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
       }
     }
     if (first_iter) UNI_FETCH(g + nwarps);
-    if (DL && pend_rec) { *(unsigned long long*)pend_rec = (unsigned long long)pend_link; pend_rec = 0ull; }
     if (created && q == 0) new_keys++;
     // ---- what does the other side hold for the key ?
     const unsigned long long WI = shfl64m(0xffffffffu, pv.y, qlead);
-    uint32_t cnt;
+    uint32_t cnt, own_cnt = 0u;  // own_cnt: the chained side's count as loaded with the bucket (0 after a claim)
     bool fast = false;
     if (!IS_ROW) {
       const uint32_t inull = __shfl_sync(0xffffffffu, (uint32_t)(pv.x & 0xffull), qlead + 1);
+      if (!PROBE_ONLY) own_cnt = __shfl_sync(0xffffffffu, (uint32_t)(pv.y >> 32), qlead + 1);
       cnt = found ? W_count(WI) : 0u;
       fast = cnt == 1u && W_istate(WI) == 1u && inull == 0u;
     } else {
@@ -499,14 +500,16 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
     }
     // ---- emit
     if (fast) {  // one match, in the bucket's inline record: the quad writes the row
-      any_match = true;
+      seen |= SEEN_MATCH;
       if (q == 0) o.ops[pos] = ins ? RW_OP_INSERT : RW_OP_DELETE;
       if (q == 1) o.vis[pos] = 1;
+      unsigned long long* const po0 = *(unsigned long long* volatile*)&s_po[q];  // (volatile: not hoisted out of the loop)
+      unsigned long long* const po1 = *(unsigned long long* volatile*)&s_po[4 + q];
       if (po0) po0[pos] = q < 2 ? va : pv.x;
       if (po1) po1[pos] = q < 2 ? vb : pv.y;
     } else if (in && q == 0) {
       // deferred rows get their visibility from uni_tail_kernel's deferred phase; the others are holes
-      if (!(act && (!keyok || cnt > 0u))) { o.vis[pos] = 0; any_hole = true; }
+      if (!(act && (!keyok || cnt > 0u))) { o.vis[pos] = 0; seen |= SEEN_HOLE; }
     }
     const bool defer = act && !fast && (!keyok || cnt > 0u);
     // extra-match rows: one reservation per warp and U_XCHUNK rows (an atomic per row on the shared counter
@@ -526,7 +529,7 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
         if ((int64_t)total > xend - xnext) {
           // leftover of the old reservation becomes invisible filler
           for (int64_t f = xnext + lane; f < xend; f += 32) { o.ops[xarea + f] = RW_OP_INSERT; o.vis[xarea + f] = 0; }
-          if (xend > xnext) any_hole = true;
+          if (xend > xnext) seen |= SEEN_HOLE;
           const uint32_t take = total > U_XCHUNK ? total : U_XCHUNK;
           unsigned long long nb = 0;
           if (lane == 0) nb = atomicAdd(&st->out_rows, (unsigned long long)take);
@@ -547,8 +550,8 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
     // ---- worklist: one mask byte per group of 8 rows (always written), an entry per deferred row
     {
       const unsigned dbal = __ballot_sync(0xffffffffu, defer && q == 0);
-      if (dbal) any_defer = true;
-      if (__any_sync(0xffffffffu, defer && !keyok)) any_sentinel = true;  // whole rows (insert included) go to the tail kernel
+      if (dbal) seen |= SEEN_DEFER;
+      if (__any_sync(0xffffffffu, defer && !keyok)) seen |= SEEN_SENTINEL;  // whole rows (insert included) go to the tail kernel
       if (lane == 0 && g * 8 < n_rows) {
         unsigned m8 = 0;
 #pragma unroll
@@ -608,6 +611,7 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
         } else {
           pool_next += k;
         }
+        seen |= SEEN_POOL;
       }
       uint32_t link = 0u;
       unsigned long long recp = 0;  // 0 = nothing to write; bit 0 set = the bucket's inline record
@@ -624,18 +628,9 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
           recp = (unsigned long long)useg_rec(own.log, row);
         }
       } else if (row != U_NIL) {
-        link = atomicExch((uint32_t*)(buckets + idx * 64 + 24), row);
-        atomicAdd((uint32_t*)(buckets + idx * 64 + 28), 1u);
+        link = uni_chain_push((unsigned long long*)(buckets + idx * 64 + 24), row, own_cnt);
         recp = (unsigned long long)useg_rec(own.log, row);
       }
-      if (DL && !IS_ROW) {
-        if (q == 0 && recp) { pend_rec = recp; pend_link = link; }  // (the link is still in flight: not touched here)
-        recp = shfl64m(0xffffffffu, recp, qlead);
-        if (recp && q != 0) {
-          if (q == 1) *(unsigned long long*)(recp + 8) = seq_base + (unsigned long long)r;  // the link word follows later
-          else *(ulonglong2*)(recp + 16 * (q - 1)) = make_ulonglong2(va, vb);
-        }
-      } else {
       recp = shfl64m(0xffffffffu, recp, qlead);
       link = __shfl_sync(0xffffffffu, link, qlead);
       if (recp && q != 0) {
@@ -651,19 +646,17 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
           *(ulonglong2*)(recp + 16 * (q - 1)) = v;
         }
       }
-      }
     }
   }
 #undef UNI_FETCH
-  if (DL && pend_rec) *(unsigned long long*)pend_rec = (unsigned long long)pend_link;
   // leftover of the extra-row reservation
   for (int64_t f = xnext + lane; f < xend; f += 32) { o.ops[xarea + f] = RW_OP_INSERT; o.vis[xarea + f] = 0; }
-  if (xend > xnext) any_hole = true;
-  if (!PROBE_ONLY && lane == 0 && (pool_next != pool_next0 || pool_end != pool_end0)) own.pools[warp_global] = make_uint2(pool_next, pool_end);
-  unsigned long long flags = (any_hole ? (1ull << 63) : 0ull);
-  const bool warp_match = __any_sync(0xffffffffu, any_match);
-  const bool warp_defer = __any_sync(0xffffffffu, any_defer);
-  const bool warp_sentinel = __any_sync(0xffffffffu, any_sentinel);
+  if (xend > xnext) seen |= SEEN_HOLE;
+  if (!PROBE_ONLY && lane == 0 && (seen & SEEN_POOL)) own.pools[warp_global] = make_uint2(pool_next, pool_end);
+  unsigned long long flags = ((seen & SEEN_HOLE) ? (1ull << 63) : 0ull);
+  const bool warp_match = __any_sync(0xffffffffu, (seen & SEEN_MATCH) != 0u);
+  const bool warp_defer = __any_sync(0xffffffffu, (seen & SEEN_DEFER) != 0u);
+  const bool warp_sentinel = __any_sync(0xffffffffu, (seen & SEEN_SENTINEL) != 0u);
   for (int d = 16; d > 0; d >>= 1) {
     flags |= __shfl_xor_sync(0xffffffffu, flags, d);
     new_keys += __shfl_xor_sync(0xffffffffu, new_keys, d);

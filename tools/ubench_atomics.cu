@@ -43,6 +43,14 @@ __global__ void k(ulonglong2* tab, uint64_t mask, uint64_t n, uint64_t seed, uns
       v.x += 1; v.y += 1;
       *p = v;
     }
+    if (MODE == 13) {  // load16, then ONE EXCH64 of head | (count + 1) << 32; RED only when the count moved meanwhile (insert)
+      ulonglong2 v = __ldcg(p);
+      const unsigned int L = (unsigned int)(v.y >> 32);
+      const unsigned long long old = atomicExch((unsigned long long*)p + 1, (unsigned long long)(unsigned int)i | ((unsigned long long)(L + 1u) << 32));
+      const unsigned int C = (unsigned int)(old >> 32);
+      if (C != L) atomicAdd((unsigned int*)p + 3, C - L);
+      acc += (unsigned int)old + v.x;
+    }
   }
   if (acc == 0x1234567) *sink = acc;
 }
@@ -80,6 +88,7 @@ int main() {
     run<2>("ATOM.EXCH u32", tab, slots, n, sink);
     run<3>("ATOM.CAS u64", tab, slots, n, sink);
     run<4>("load16 + EXCH32 + RED32 (insert)", tab, slots, n, sink);
+    run<13>("load16 + EXCH64 (+RED if moved)", tab, slots, n, sink);
     run<6>("3x RED u64 one slot (agg)", tab, slots, n, sink);
     run<9>("load -> CAS64 + CAS32 + ADD32", tab, slots, n, sink);
     run<10>("load -> CAS64", tab, slots, n, sink);
