@@ -20,9 +20,13 @@
 //                  bounds this workload; tools/ubench_atomics.cu measures their rate.)
 //   overflow store: further rows of a key go to an append-only array of records chained through
 //                  `link` from the bucket's head.
-// Two execution paths:
-//   * inner fast path (no degrees): ONE fused kernel per batch -- probe the other side, emit the
-//     matches with tile-scan compaction, append the row to the own side; a second kernel applies
+// Three execution paths, chosen by the plan (and, within a path, by whether the chunk carries bitmaps):
+//   * unified table (join_uni.cuh): Key64 inner joins with <= 4 eight-byte columns per side keep BOTH
+//     sides in one bucket array, so a row's probe and its own-side insert touch the same line.
+//   * two-table inner kernels (no degrees): ONE kernel per batch probes the other side, emits the
+//     matches and appends the row to the own side -- join_inner_w8p_kernel for Key64 with 5-8
+//     eight-byte columns (chunks without bitmaps), join_inner_fused_kernel (tile-scan compaction)
+//     for typed or multi-key plans and chunks with bitmaps; join_inner_delete_kernel then applies
 //     own-side deletes (it exits immediately when the batch has none).
 //   * generic path (all 8 join types, degrees, append-only optimisation, mixed +/- on one key):
 //     the batch is grouped by join key (scratch hash table + radix sort) and ONE thread walks each
@@ -100,8 +104,6 @@ struct JoinSideDev {
   uint8_t* recs;     // overflow record store
   uint8_t* buckets;  // hash index with inline records
   uint64_t cap;
-  uint2* pools;      // per-warp row-id pools of the overflow store {next, end} (join_inner_q4_kernel)
-  uint64_t rec_cap;  // records the overflow store can hold
   int stride;
   int bstride;
 };
@@ -194,8 +196,7 @@ __device__ __forceinline__ uint64_t key_hash(const JoinPlanDev* p, const uint64_
 }
 
 // Key64 tables: the probe sequence of a key starts at an EVEN bucket, i.e. at a 128-byte aligned pair
-// of 64-byte buckets, and continues bucket by bucket.  The quad-cooperative kernel fetches the whole
-// pair with one 32-byte load per lane: the second probe of a collision costs no second trip to HBM.
+// of 64-byte buckets, and continues bucket by bucket.
 __device__ __forceinline__ uint64_t home64(uint64_t key, uint64_t mask) { return mix64(key) & mask & ~1ull; }
 
 // bucket = [key word(s)] [state word W] [inline record]
@@ -846,7 +847,6 @@ __global__ void __launch_bounds__(JF_BLOCK, 8) join_inner_fused_kernel(const Joi
 // Rows it cannot take (key == EMPTY sentinel, matched record with NULLs, keys with several rows)
 // fall through to the same helpers the generic kernel uses.
 #define W8_MAXC 8
-#define Q4_MAX_GRID (RW_SMS * 8)  // blocks of JF_BLOCK threads; one row-id pool per warp
 struct W8Plan {
   int n_u, n_m;            // columns of the update / matched side (all 8 bytes wide)
   int key_col;             // key column of the update side
@@ -1046,297 +1046,6 @@ __global__ void __launch_bounds__(JF_BLOCK, 4) join_inner_w8p_kernel(const JoinP
   }
 }
 
-// a chunk whose row count lives on the device (e.g. the output of the exchange): clamp the capacity
-__device__ __forceinline__ int64_t chunk_rows(const DevChunk& ch, JoinStatus* st, bool report) {
-  if (!ch.n_dev) return ch.n;
-  const int64_t n = *ch.n_dev;
-  if (n < 0 || n > ch.n) {
-    if (report) atomicOr(&st->err, JERR_BAD_COUNT);
-    return 0;
-  }
-  if (report) st->n_in = (unsigned long long)n;
-  return n;
-}
-
-// ------------------------------------------------------------------ quad-cooperative Key64 kernel (<= 4 + 4 columns)
-// tools/ubench_bucket.cu: what a random bucket access costs is the number of memory INSTRUCTIONS that
-// touch the line, not its bytes -- one thread reading a 64-byte bucket with 4 x LDG.128 costs several
-// times what four lanes reading 16 bytes each in ONE instruction cost (the price of a single 16-byte
-// load); a record written with three 16-byte stores is cheap once the claiming CAS has pulled the line
-// into L2.
-// So a row is owned by a QUAD of lanes and a warp works on 8 rows:
-//   lane q of the quad loads piece q of the other side's bucket   [key|W] [rec hdr] [col0,col1] [col2,col3]
-//   lanes 0,1 hold the update row's columns (0,1) / (2,3) and write them to the output,
-//   lanes 2,3 hold the matched columns and write those -- two store instructions emit the row;
-//   lane 0 claims the own-side bucket with one speculative 128-bit CAS issued BEFORE the probe
-//   resolves (both random accesses are in flight together); lanes 1..3 then write the record
-//   (header, columns) with one 16-byte store each into the line the CAS just brought in.
-// Rows the quad cannot finish this way (sentinel key, several matches, match not in the inline
-// record, NULLs in the matched record) are finished by lane 0 with the generic helpers.
-// Output convention: positional, exactly as join_inner_w8p_kernel.
-struct U256 { uint64_t a, b, c, d; };
-// 32 bytes of one sector, L2 only: sm_90 has no 256-bit load, so two 16-byte loads issued back to back
-// (both in flight together; the second hits the sector the first one requested)
-__device__ __forceinline__ U256 ld256_cg(const void* ptr) {
-  U256 v;
-  asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
-               : "=l"(v.a), "=l"(v.b), "=l"(v.c), "=l"(v.d) : "l"(ptr));
-  return v;
-}
-__device__ __forceinline__ uint64_t shfl64m(unsigned mask, uint64_t v, int src) {
-  return (uint64_t)__shfl_sync(mask, (unsigned long long)v, src);
-}
-
-template <bool PROBE_ONLY, int MINB>
-__global__ void __launch_bounds__(JF_BLOCK, MINB) join_inner_q4_kernel(const JoinPlanDev* __restrict__ p, W8Plan w, int S, DevChunk ch,
-                                                                     JoinSideDev own, JoinSideDev other, JoinOutDev o, JoinStatus* st,
-                                                                     uint32_t store_base, uint64_t seq_base, int64_t out_base, uint32_t pool_chunk) {
-  // (kept in a register: writing ch.n would force a local-memory copy of the whole parameter struct)
-  const int64_t n_rows = chunk_rows(ch, st, blockIdx.x == 0 && threadIdx.x == 0);
-  const int lane = lane_id(), q = lane & 3, qlead = lane & ~3;
-  // Overflow row ids come from a per-warp pool that persists across launches: one atomicAdd on the
-  // shared counter hands a warp `pool_chunk` ids.  (One atomicAdd per 8 rows on that single address
-  // was slower -- same-address atomics serialise in one L2 slice.)
-  const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  uint32_t pool_next = 0, pool_end = 0;
-  if (!PROBE_ONLY) {
-    const uint2 pl = own.pools[warp_global];
-    pool_next = pl.x;
-    pool_end = pl.y;
-  }
-  const uint32_t pool_next0 = pool_next, pool_end0 = pool_end;
-  const uint64_t omask = other.cap - 1, wmask = own.cap - 1;
-  unsigned int new_keys = 0, n_del = 0;
-  bool any_match = false, any_hole = false;
-  // column roles of this lane
-  const int ca = 2 * (q & 1), cb = ca + 1;
-  const unsigned long long* pa = ca < w.n_u ? (const unsigned long long*)ch.cols[ca].data : nullptr;
-  const unsigned long long* pb = cb < w.n_u ? (const unsigned long long*)ch.cols[cb].data : nullptr;
-  const unsigned long long* pk = (const unsigned long long*)ch.cols[w.key_col].data;
-  int oc0, oc1;
-  if (q < 2) {
-    oc0 = ca < w.n_u ? w.u_out[ca] : -1;
-    oc1 = cb < w.n_u ? w.u_out[cb] : -1;
-  } else {
-    oc0 = ca < w.n_m ? w.m_out[ca] : -1;
-    oc1 = cb < w.n_m ? w.m_out[cb] : -1;
-  }
-  uint64_t* po0 = oc0 >= 0 ? (uint64_t*)o.col[oc0] : nullptr;
-  uint64_t* po1 = oc1 >= 0 ? (uint64_t*)o.col[oc1] : nullptr;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int64_t groups = (n_rows + 7) >> 3;
-  ulonglong2 cas_empty, cas_want;
-  cas_empty.x = J_EMPTY;
-  cas_empty.y = W_EMPTY;
-  cas_want.y = (W_EMPTY | W_IL_LIVE) + W_COUNT_ONE;
-  // All shuffles use the full-warp mask and sit in warp-uniform control flow: a shuffle with a
-  // per-quad mask splits the warp into eight separately issued groups.
-  // Software pipeline: the (sequential) column loads of the warp's NEXT group are issued right after
-  // the random accesses of the current one, so they are out of the dependent chain
-  // ops -> key -> bucket / CAS -> chain CAS that bounds this latency-bound kernel.
-  uint8_t n_op = 0;
-  uint64_t n_key = J_EMPTY, n_va = 0ull, n_vb = 0ull;
-  auto fetch = [&](int64_t g2) {
-    const int64_t r2 = g2 * 8 + (lane >> 2);
-    n_op = 0;
-    if (g2 < groups && r2 < n_rows) {
-      n_op = ch.ops[r2];
-      n_key = __ldg(pk + r2);
-      if (pa) n_va = __ldg(pa + r2);
-      if (pb) n_vb = __ldg(pb + r2);
-    }
-  };
-  fetch(warp_global);
-  for (int64_t g = warp_global; g < groups; g += nwarps) {
-    const int64_t r = g * 8 + (lane >> 2);
-    const bool in = r < n_rows;
-    const uint8_t op = n_op;
-    const uint64_t key = n_key, va = n_va, vb = n_vb;
-    const int64_t pos = out_base + r;
-    const bool act = op != 0;
-    if (in && !act) {  // invisible input row
-      if (q == 0) o.vis[pos] = 0;
-      any_hole = true;
-    }
-    const bool ins = act && (op == RW_OP_INSERT || op == RW_OP_UPDATE_INSERT);
-    if (act && !ins && q == 0) n_del++;
-    const bool keyok = act && key != J_EMPTY;
-    const uint64_t hsh = mix64(key);
-    // ---- own side: speculative claim, in flight together with the probe
-    const bool do_ins = !PROBE_ONLY && ins;
-    // (the result `cf` is only looked at after the probe: comparing it here would make the warp
-    // wait for the atomic before the probe load is even issued)
-    ulonglong2 cf;
-    cf.x = 0; cf.y = 0;
-    uint64_t widx = hsh & wmask & ~1ull;
-    if (do_ins && keyok && q == 0) {
-      cas_want.x = key;
-      cas128(own.buckets + widx * 64, cas_empty, cas_want, &cf);
-    }
-    fetch(g + nwarps);
-    // ---- probe: the quad fetches the 128-byte bucket PAIR, one 32-byte load per lane
-    //   lane 0: A.key A.W A.hdr   lane 1: A.cols 0..3   lane 2: B.key B.W B.hdr   lane 3: B.cols 0..3
-    // the warp iterates until its longest probe sequence ends (finished quads idle)
-    bool found = false, need = keyok;
-    uint64_t idx = hsh & omask & ~1ull;
-    int sel = 0;  // 0: matched bucket A, 2: bucket B
-    U256 pv;
-    pv.a = 0; pv.b = 0; pv.c = 0; pv.d = 0;
-    while (__any_sync(0xffffffffu, need)) {
-      if (need) pv = ld256_cg(other.buckets + idx * 64 + 32 * q);
-      const uint64_t kA = shfl64m(0xffffffffu, pv.a, qlead), kB = shfl64m(0xffffffffu, pv.a, qlead + 2);
-      if (need) {
-        if (kA == key) { found = true; sel = 0; need = false; }
-        else if (kB == key) { found = true; sel = 2; need = false; }
-        else if (kA == J_EMPTY || kB == J_EMPTY) need = false;  // an empty bucket ends the probe sequence
-        else idx = (idx + 2) & omask;
-      }
-    }
-    const int hl = qlead + sel;  // lane holding key | W | record header of the matched bucket
-    const uint64_t W = shfl64m(0xffffffffu, pv.b, hl);
-    const uint32_t mnull = __shfl_sync(0xffffffffu, (uint32_t)(pv.c >> 32), hl);  // rec hdr: link | nullmask
-    // matched columns: lane 2 writes (0,1), lane 3 writes (2,3)
-    const uint64_t m0 = shfl64m(0xffffffffu, pv.a, hl + 1), m1 = shfl64m(0xffffffffu, pv.b, hl + 1);
-    const uint64_t m2 = shfl64m(0xffffffffu, pv.c, hl + 1), m3 = shfl64m(0xffffffffu, pv.d, hl + 1);
-    const uint64_t ma = q == 3 ? m2 : m0, mb = q == 3 ? m3 : m1;
-    // ---- emit
-    uint32_t cnt = found ? W_count(W) : 0u;
-    if (cnt == 1u && W_istate(W) == 1u && mnull == 0u) {
-      any_match = true;
-      if (q == 0) o.ops[pos] = ins ? RW_OP_INSERT : RW_OP_DELETE;
-      if (q == 1) o.vis[pos] = 1;
-      if (po0) po0[pos] = q < 2 ? va : ma;
-      if (po1) po1[pos] = q < 2 ? vb : mb;
-    } else if (act && q == 0) {
-      int64_t ob = found ? (int64_t)idx + (sel >> 1) : -1;
-      if (!keyok) {
-        uint64_t kw[1] = {key}, hc = 0;
-        ob = js_find(other, p, kw, 0, &hc);
-        cnt = ob >= 0 ? W_count(hc) : 0u;
-      }
-      if (cnt == 0u) {
-        o.vis[pos] = 0;
-        any_hole = true;
-      } else {
-        any_match = true;
-        o.vis[pos] = 1;
-        const uint8_t oop = ins ? RW_OP_INSERT : RW_OP_DELETE;
-        uint32_t left = cnt;
-        int64_t xpos = 0;
-        if (cnt > 1u) {
-          xpos = out_base + n_rows + (int64_t)atomicAdd(&st->out_rows, (unsigned long long)(cnt - 1));
-          if (xpos + (cnt - 1) > o.capacity) { atomicOr(&st->err, JERR_OUT_CAPACITY); left = 1; }
-        }
-        bool first = true;
-        for_each_live(other, p, ob, [&](uint8_t* mrec) -> bool {
-          int64_t at = pos;
-          if (!first) { o.vis[xpos] = 1; at = xpos++; }
-          first = false;
-          emit_row(o, p, st, at, oop, S, ch, r, mrec);
-          return --left != 0;
-        });
-      }
-    }
-    // ---- append to the own side
-    uint64_t recp = 0;
-    uint32_t link = 0u;
-    bool need_ovf = false;
-    unsigned long long Wcur = 0ull;
-    unsigned long long* Wp = nullptr;
-    if (do_ins && q == 0) {
-      bool created = false, inline_won = false;
-      if (keyok) {
-        while (true) {
-          if (cf.x == J_EMPTY && cf.y == W_EMPTY) { created = true; inline_won = true; break; }  // the CAS took the bucket
-          if (cf.x == key) { Wcur = cf.y; break; }
-          widx = (widx + 1) & wmask;  // bucket held by another key
-          cas128(own.buckets + widx * 64, cas_empty, cas_want, &cf);
-        }
-        Wp = (unsigned long long*)(own.buckets + widx * 64 + 8);
-      } else {
-        uint64_t kw[1] = {key};
-        widx = (uint64_t)js_find_or_insert(own, p, kw, 0, &created);
-        Wp = (unsigned long long*)(own.buckets + widx * 64 + 8);
-        Wcur = __ldcg(Wp);
-      }
-      if (created) new_keys++;
-      if (!inline_won) {
-        while (W_istate(Wcur) != 1u) {  // the inline record is free (never used, or its row was deleted)
-          const unsigned long long nw = ((Wcur & ~W_IL_MASK) | W_IL_LIVE) + W_COUNT_ONE;
-          const unsigned long long old = atomicCAS(Wp, Wcur, nw);
-          if (old == Wcur) { inline_won = true; break; }
-          Wcur = old;
-        }
-      }
-      if (inline_won) recp = (uint64_t)(own.buckets + widx * 64 + 16);
-      else need_ovf = true;
-    }
-    if (!PROBE_ONLY) {
-      const unsigned bal = __ballot_sync(0xffffffffu, need_ovf);
-      if (bal) {  // warp-uniform: ids for the rows that go to the overflow store
-        const uint32_t k = __popc(bal), left = pool_end - pool_next;
-        uint32_t nb = 0;
-        if (left < k) {  // refill; the remainder of the old chunk is used up first
-          if (lane == 0) {
-            nb = store_base + (uint32_t)atomicAdd(&st->n_store, (unsigned long long)pool_chunk);
-            if ((uint64_t)nb + pool_chunk > own.rec_cap) { atomicOr(&st->err, JERR_STORE_CAPACITY); nb = 0xffffffffu; }
-          }
-          nb = __shfl_sync(0xffffffffu, nb, 0);
-        }
-        const uint32_t i = __popc(bal & ((1u << lane) - 1u));
-        const uint32_t row = i < left ? pool_next + i : nb + (i - left);
-        const bool bad = left < k && nb == 0xffffffffu;
-        if (left < k) {
-          pool_next = bad ? 0u : nb + (k - left);
-          pool_end = bad ? 0u : nb + pool_chunk;
-        } else {
-          pool_next += k;
-        }
-        if (need_ovf && !(bad && i >= left)) {
-          while (true) {  // one CAS pushes the row on the key's chain
-            const unsigned long long nw = ((Wcur & ~0x7fffffffull) | (unsigned long long)row) + W_COUNT_ONE;
-            const unsigned long long old = atomicCAS(Wp, Wcur, nw);
-            if (old == Wcur) break;
-            Wcur = old;
-          }
-          link = W_head(Wcur);
-          recp = (uint64_t)rec_ptr(own, row);
-        }
-      }
-      recp = shfl64m(0xffffffffu, recp, qlead);
-      link = __shfl_sync(0xffffffffu, link, qlead);
-      if (do_ins && q != 0 && recp) {
-        ulonglong2 v;
-        if (q == 1) {  // RecHdr {link, nullmask = 0, seq, degree = 0}
-          v.x = (unsigned long long)link;
-          v.y = (unsigned long long)(seq_base + (uint64_t)r);  // {seq, degree} = the 64-bit arrival number
-        } else {       // lane 2: columns 0,1   lane 3: columns 2,3
-          v.x = va;
-          v.y = vb;
-        }
-        *(ulonglong2*)(recp + 16 * (q - 1)) = v;
-      }
-    }
-  }
-  if (!PROBE_ONLY && lane == 0 && (pool_next != pool_next0 || pool_end != pool_end0)) own.pools[warp_global] = make_uint2(pool_next, pool_end);
-  unsigned long long flags = (any_hole ? (1ull << 63) : 0ull);
-  const bool warp_match = __any_sync(0xffffffffu, any_match);
-  for (int d = 16; d > 0; d >>= 1) {
-    flags |= __shfl_xor_sync(0xffffffffu, flags, d);
-    new_keys += __shfl_xor_sync(0xffffffffu, new_keys, d);
-    n_del += __shfl_xor_sync(0xffffffffu, n_del, d);
-  }
-  if (lane == 0) {
-    if (flags && (__ldcg(&st->null_mask) & flags) != flags) atomicOr(&st->null_mask, flags);
-    if (warp_match && __ldcg(&st->pad) == 0u) st->pad = 1u;
-    if (!PROBE_ONLY && new_keys) atomicAdd(&st->n_keys[S], (unsigned long long)new_keys);
-    if (!PROBE_ONLY && n_del) atomicAdd(&st->n_del, (unsigned long long)n_del);
-  }
-}
-
-// own-side deletes of the fast path (after the fused kernel; exits at once when the batch has none).
-// Sequential rule: the delete at chunk position r removes the live record with equal pk that
-// arrived most recently BEFORE r (64-bit arrival numbers, see the kernel).
 // status block -> pinned host memory (UVA), tagged so the host can tell a fresh copy from a stale one;
 // then the per-push counters are zeroed for the next push (reset bit 0: n_store / n_del / null_mask,
 // bit 1: out_rows / pad of the positional kernels).
@@ -1349,10 +1058,13 @@ __device__ __forceinline__ void join_status_publish(JoinStatus* st, JoinStatus* 
   if (reset & 2) { st->out_rows = 0ull; st->pad = 0u; st->n_in = 0ull; }
 }
 
+// own-side deletes of the two-table inner kernels (launched behind them; exits at once when the batch has none).
+// Sequential rule: the delete at chunk position r removes the live record with equal pk that
+// arrived most recently BEFORE r (64-bit arrival numbers, see the loop).
 __global__ void __launch_bounds__(256) join_inner_delete_kernel(const JoinPlanDev* __restrict__ p, int S, DevChunk ch,
                                                                  JoinSideDev own, JoinStatus* st, uint64_t seq_base,
                                                                  JoinStatus* status_host, unsigned long long tag, int reset) {
-  const int64_t n_rows = chunk_rows(ch, st, false);
+  const int64_t n_rows = ch.n;  // never counted on the device: the host reads a device-resident count back first
   if (*(volatile unsigned long long*)&st->n_del == 0ull) {
     // nothing to delete (the usual case): this launch doubles as the status read-back
     if (status_host && blockIdx.x == 0 && threadIdx.x == 0) join_status_publish(st, status_host, tag, reset);
@@ -1779,7 +1491,7 @@ struct JoinSideHost {
   SegLog log;          // unified table: the side's row log
   GrowBuf recs;        // overflow record store (grows in place)
   DevBuf slots;        // bucket array
-  DevBuf pools;        // per-warp row-id pools of join_inner_q4_kernel
+  DevBuf pools;        // unified table: per-warp row-id pools of the side's log (uni_hot_kernel)
   int stride = 0, bstride = 0;
   uint64_t row_cap = 0;   // records allocated
   uint64_t n_rows = 0;    // records handed out (incl. dead ones)
@@ -1812,7 +1524,6 @@ struct rwgpu_join {
   int chunk_size = 1024;
   bool fast_inner = false;
   bool w8_ok[2] = {false, false};  // per update side: Key64 + all-8-byte columns specialisation usable
-  bool q4_ok = false;              // both sides: 3..4 columns, 64-byte buckets -> quad-cooperative kernel
   W8Plan w8[2];
   // unified table (join_uni.cuh): Key64 inner join, <= 4 eight-byte columns per side -- ONE bucket array for both sides
   bool uni = false;
@@ -1907,8 +1618,6 @@ static JoinSideDev side_dev(const rwgpu_join* h, int S) {
   const JoinSideHost& s = h->side[S];
   JoinSideDev d;
   d.recs = s.recs.as<uint8_t>();
-  d.pools = s.pools.as<uint2>();
-  d.rec_cap = s.row_cap;
   d.buckets = s.slots.as<uint8_t>();
   d.cap = s.slot_cap;
   d.stride = s.stride;
@@ -2227,22 +1936,9 @@ static int uni_launch_main(rwgpu_join* h, const JoinPending& pd, bool probe_only
       po.mcol[c] = (c < w.n_m && w.m_out[c] >= 0) ? (unsigned long long*)od.col[w.m_out[c]] : nullptr;
     }
     po.capacity = od.capacity;
-    // resident blocks per SM (registers per thread): 4 (64) by default; RWGPU_UNI_MINB=3 / 5 / 6 for tuning runs
-    static const int minb = getenv("RWGPU_UNI_MINB") ? atoi(getenv("RWGPU_UNI_MINB")) : 4;
-#define UNI_LAUNCH(PO, IS, MB) uni_hot_kernel<PO, IS, MB><<<pd.grid, JF_BLOCK, 0, pd.st>>>(pc, t.buckets, t.cap, own, po, wk, ds, pd.seq_base, pd.out_base, pd.pool_chunk)
-    if (probe_only) {
-      if (is_row) UNI_LAUNCH(true, true, 4); else UNI_LAUNCH(true, false, 4);
-    } else if (is_row) {
-      UNI_LAUNCH(false, true, 4);
-    } else {
-      switch (minb) {
-        case 3: UNI_LAUNCH(false, false, 3); break;
-        case 5: UNI_LAUNCH(false, false, 5); break;
-        case 6: UNI_LAUNCH(false, false, 6); break;
-        default: UNI_LAUNCH(false, false, 4); break;
-      }
-    }
-#undef UNI_LAUNCH
+    auto hot = probe_only ? (is_row ? uni_hot_kernel<true, true> : uni_hot_kernel<true, false>)
+                          : (is_row ? uni_hot_kernel<false, true> : uni_hot_kernel<false, false>);
+    hot<<<pd.grid, JF_BLOCK, 0, pd.st>>>(pc, t.buckets, t.cap, own, po, wk, ds, pd.seq_base, pd.out_base, pd.pool_chunk);
   } else {
     if (probe_only) uni_slow_kernel<true><<<jgrid(pd.ch.n, 256), 256, 0, pd.st>>>(pdev, w, S, pd.ch, t, od, ds, pd.seq_base, pd.out_base);
     else uni_slow_kernel<false><<<jgrid(pd.ch.n, 256), 256, 0, pd.st>>>(pdev, w, S, pd.ch, t, od, ds, pd.seq_base, pd.out_base);
@@ -2264,6 +1960,23 @@ static int uni_launch_main(rwgpu_join* h, const JoinPending& pd, bool probe_only
   return RW_OK;
 }
 
+// *plain: the chunk carries no bitmaps (ops == 0 still hides rows), which the Key64 / 8-byte-column kernels need.
+// Only uni_hot_kernel reads a device-resident row count on the device: unless `device_count` allows that and the
+// chunk is plain, the count is read back (one 8-byte copy) and the chunk becomes an ordinary one.
+static int join_plain_chunk(DevChunk* ch, bool device_count, cudaStream_t st, bool* plain) {
+  *plain = ch->vis_bits == nullptr;
+  for (int c = 0; c < ch->n_cols && *plain; c++)
+    *plain = !ch->cols[c].valid_bits && !ch->cols[c].valid_bytes && (((uintptr_t)ch->cols[c].data & 7) == 0);
+  if (!ch->n_dev || (device_count && *plain)) return RW_OK;
+  int64_t nh = 0;
+  RW_CUDA(cudaMemcpyAsync(&nh, ch->n_dev, sizeof(nh), cudaMemcpyDeviceToHost, st));
+  RW_CUDA(cudaStreamSynchronize(st));
+  if (nh < 0 || nh > ch->n) return fail(RW_ERR_INVALID, "device row count out of range");
+  ch->n = nh;
+  ch->n_dev = nullptr;
+  return RW_OK;
+}
+
 // LAUNCH half of a push: main kernel + delete kernel (which publishes the status block into the output set's pinned
 // slot) are enqueued on `st`; nothing is waited for.  The output goes to the CURRENT output set (h->cur).
 static double uni_now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
@@ -2272,28 +1985,19 @@ static const bool uni_trace = getenv("RWGPU_TRACE") != nullptr;  // host-side ti
 static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t st, int64_t out_base, JoinPending* pd) {
   const double tr0 = uni_trace ? uni_now_ms() : 0.0;
   DevChunk ch = ch_in;
-  bool plain_cols = ch.vis_bits == nullptr;
-  for (int c = 0; c < ch.n_cols && plain_cols; c++)
-    plain_cols = !ch.cols[c].valid_bits && !ch.cols[c].valid_bytes && (((uintptr_t)ch.cols[c].data & 7) == 0);
-  bool counted = ch.n_dev != nullptr;
-  if (counted && !plain_cols) {  // only the quad-cooperative kernel reads the row count on the device
-    int64_t nh = 0;
-    RW_CUDA(cudaMemcpyAsync(&nh, ch.n_dev, sizeof(nh), cudaMemcpyDeviceToHost, st));
-    RW_CUDA(cudaStreamSynchronize(st));
-    if (nh < 0 || nh > ch.n) return fail(RW_ERR_INVALID, "device row count out of range");
-    ch.n = nh;
-    ch.n_dev = nullptr;
-    counted = false;
-  }
+  bool plain_cols;
+  int rc = join_plain_chunk(&ch, true, st, &plain_cols);
+  if (rc != RW_OK) return rc;
+  const bool counted = ch.n_dev != nullptr;
   const int64_t n = ch.n;  // capacity when `counted`
   JoinSideHost& own = h->side[S];
-  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 63) / 64, Q4_MAX_GRID));
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 63) / 64, U_MAX_GRID));
   uint32_t pool_chunk = 32;
   while (pool_chunk < 256 && (int64_t)pool_chunk * grid * 8 < 4 * n) pool_chunk <<= 1;
   // the warps draw log ids from persistent pools in chunks: the id counter can run ahead of the rows stored by one chunk
   // per warp.  own.n_rows / uni_keys are UPPER bounds while pushes are outstanding (corrected when they are collected).
   const uint64_t id_slack = (uint64_t)grid * 8 * pool_chunk;
-  int rc = join_grow_store(h, S, own.n_rows + (uint64_t)n + id_slack);
+  rc = join_grow_store(h, S, own.n_rows + (uint64_t)n + id_slack);
   if (rc != RW_OK) return rc;
   rc = uni_grow_table(h, h->uni_keys + (uint64_t)n);
   if (rc != RW_OK) return rc;
@@ -2325,8 +2029,7 @@ static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t
   h->seq += (uint64_t)n;
   own.n_rows += (uint64_t)n + id_slack;  // upper bounds until the status comes back
   h->uni_keys += (uint64_t)n;
-  static const bool dbg_probe_only = getenv("RWGPU_DBG_PROBE_ONLY") != nullptr;  // timing experiments only (state is not updated)
-  rc = uni_launch_main(h, *pd, dbg_probe_only && S == 0, pd->tag);
+  rc = uni_launch_main(h, *pd, false, pd->tag);
   if (rc != RW_OK) return rc;
   if (!h->pend_ev[pd->set]) RW_CUDA(cudaEventCreateWithFlags(&h->pend_ev[pd->set], cudaEventDisableTiming));
   RW_CUDA(cudaEventRecord(h->pend_ev[pd->set], st));
@@ -2428,37 +2131,18 @@ static int join_push_dev(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream
   if (ch.n <= 0) return RW_OK;
   if (ch.n >= (1ll << 31)) return fail(RW_ERR_INVALID, "chunk too large");
   if (h->uni) return join_push_dev_uni(h, S, ch_in, st, out_base, out_rows, null_mask);
-  // Key64 / 8-byte-column specialisations need a chunk without bitmaps (ops == 0 still hides rows)
-  bool plain_cols = ch.vis_bits == nullptr;
-  for (int c = 0; c < ch.n_cols && plain_cols; c++)
-    plain_cols = !ch.cols[c].valid_bits && !ch.cols[c].valid_bytes && (((uintptr_t)ch.cols[c].data & 7) == 0);
-  static const bool no_q4_env = getenv("RWGPU_NO_Q4") != nullptr;
-  // device-resident row count: only the quad-cooperative kernel reads it on the device; every other path
-  // fetches it first (one 8-byte read-back) and proceeds with an ordinary chunk
-  bool counted = ch.n_dev != nullptr;
-  if (counted && !(h->fast_inner && h->q4_ok && !no_q4_env && h->w8_ok[S] && plain_cols)) {
-    int64_t nh = 0;
-    RW_CUDA(cudaMemcpyAsync(&nh, ch.n_dev, sizeof(nh), cudaMemcpyDeviceToHost, st));
-    RW_CUDA(cudaStreamSynchronize(st));
-    if (nh < 0 || nh > ch.n) return fail(RW_ERR_INVALID, "device row count out of range");
-    ch.n = nh;
-    ch.n_dev = nullptr;
-    counted = false;
-    if (nh == 0) return RW_OK;
-  }
-  const int64_t n = ch.n;  // capacity when `counted`
+  // no two-table kernel reads a device-resident row count: it is read back first
+  bool plain_cols;
+  int rc = join_plain_chunk(&ch, false, st, &plain_cols);
+  if (rc != RW_OK) return rc;
+  if (ch.n == 0) return RW_OK;  // the device-resident count was zero
+  const int64_t n = ch.n;
   JoinSideHost& own = h->side[S];
   static const bool trace = getenv("RWGPU_TRACE") != nullptr;
   auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
   const double tt0 = now();
   const uint64_t cap0 = own.slot_cap, rcap0 = own.row_cap;
-  // quad-cooperative kernel: its warps draw overflow row ids from persistent pools in chunks, so the
-  // id counter can run ahead of the rows really stored by one chunk per warp
-  const bool q4 = h->fast_inner && h->q4_ok && !no_q4_env;
-  const int q4_grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 63) / 64, Q4_MAX_GRID));
-  uint32_t pool_chunk = 32;
-  while (pool_chunk < 256 && (int64_t)pool_chunk * q4_grid * 8 < 4 * n) pool_chunk <<= 1;
-  int rc = join_grow_store(h, S, own.n_rows + (uint64_t)n + (q4 ? (uint64_t)q4_grid * 8 * pool_chunk : 0));
+  rc = join_grow_store(h, S, own.n_rows + (uint64_t)n);
   if (rc != RW_OK) return rc;
   rc = join_grow_slots(h, S, own.keys_upper + (uint64_t)n);
   if (rc != RW_OK) return rc;
@@ -2475,35 +2159,22 @@ static int join_push_dev(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream
   if (h->fast_inner) {
     // Key64 / 8-byte-column specialisation when the chunk carries no bitmaps (ops == 0 still hides rows)
     const bool use_w8 = h->w8_ok[S] && plain_cols;
-    static const bool dbg_probe_only = getenv("RWGPU_DBG_PROBE_ONLY") != nullptr;  // timing experiments only (state is not updated)
     if (use_w8) {
       // positional output: n rows aligned with the input + extra matches behind them
       // (out_rows / pad: zeroed by join_begin_call and by the previous push's status read-back)
       rc = join_ensure_out(h, out_base + n + std::max<int64_t>(n / 2, 4096), st, out_base);
       if (rc != RW_OK) return rc;
-      // quad-cooperative kernel when both sides fit a 64-byte bucket (<= 4 columns); else one thread per row
-      const int grid = q4 ? q4_grid : jgrid(n, JF_BLOCK);
+      const int grid = jgrid(n, JF_BLOCK);
       auto launch = [&](bool probe_only, uint32_t store_base) {
-        if (q4) {
-          // 4 blocks of 256 threads per SM (64 registers): the kernel is bound by random DRAM transactions, not by
-          // occupancy, and more resident blocks do not make it faster.
-          if (probe_only)
-            join_inner_q4_kernel<true, 4><<<grid, JF_BLOCK, 0, st>>>(pd, h->w8[S], S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h),
-                                                                      ds, store_base, seq_base, out_base, pool_chunk);
-          else
-            join_inner_q4_kernel<false, 4><<<grid, JF_BLOCK, 0, st>>>(pd, h->w8[S], S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h),
-                                                                       ds, store_base, seq_base, out_base, pool_chunk);
-        } else {
-          if (probe_only)
-            join_inner_w8p_kernel<true><<<grid, JF_BLOCK, 0, st>>>(pd, h->w8[S], S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h), ds,
-                                                                    store_base, seq_base, out_base);
-          else
-            join_inner_w8p_kernel<false><<<grid, JF_BLOCK, 0, st>>>(pd, h->w8[S], S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h), ds,
-                                                                     store_base, seq_base, out_base);
-        }
+        if (probe_only)
+          join_inner_w8p_kernel<true><<<grid, JF_BLOCK, 0, st>>>(pd, h->w8[S], S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h), ds,
+                                                                  store_base, seq_base, out_base);
+        else
+          join_inner_w8p_kernel<false><<<grid, JF_BLOCK, 0, st>>>(pd, h->w8[S], S, ch, side_dev(h, S), side_dev(h, 1 - S), out_dev(h), ds,
+                                                                   store_base, seq_base, out_base);
       };
       h->prof.begin(st);
-      launch(dbg_probe_only && S == 0, (uint32_t)own.n_rows);
+      launch(false, (uint32_t)own.n_rows);
       h->prof.end(st);
       const unsigned long long tag = ++h->status_tag;
       join_inner_delete_kernel<<<jgrid(n, 256), 256, 0, st>>>(pd, S, ch, side_dev(h, S), ds, seq_base, h->status_host.as<JoinStatus>(), tag, 3);
@@ -2535,8 +2206,7 @@ static int join_push_dev(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream
       hs.err = err;
       rc = join_check_err(h, hs, st);
       if (rc != RW_OK) return rc;
-      const int64_t n_eff = counted ? (int64_t)hs.n_in : n;  // positional rows = rows of the input chunk
-      *out_rows = (any_match || hs.out_rows) ? n_eff + (int64_t)hs.out_rows : 0;
+      *out_rows = (any_match || hs.out_rows) ? n + (int64_t)hs.out_rows : 0;  // positional rows = rows of the input chunk
     } else {
       rc = join_ensure_out(h, out_base + std::max<int64_t>(2 * n, 4096), st, out_base);
       if (rc != RW_OK) return rc;
@@ -2817,11 +2487,9 @@ int32_t rwgpu_join_create(const rw_join_desc* d, rwgpu_join** out) {
     }
     h->w8_ok[s2] = ok;
   }
-  h->q4_ok = h->w8_ok[0] && h->w8_ok[1] && p.bhdr == 16 && p.stride[0] == 48 && p.stride[1] == 48 && p.bstride[0] == 64 &&
-             p.bstride[1] == 64 && p.n_cols[0] <= 4 && p.n_cols[1] <= 4;
 
-  // unified table: one bucket array for both sides (join_uni.cuh).  RWGPU_NO_UNI=1 keeps the two-table kernels.
-  h->uni = h->fast_inner && h->w8_ok[0] && h->w8_ok[1] && p.n_cols[0] <= 4 && p.n_cols[1] <= 4 && getenv("RWGPU_NO_UNI") == nullptr;
+  // unified table: one bucket array for both sides (join_uni.cuh)
+  h->uni = h->fast_inner && h->w8_ok[0] && h->w8_ok[1] && p.n_cols[0] <= 4 && p.n_cols[1] <= 4;
   h->uni_is = pk_in_jk[1] ? 1 : (pk_in_jk[0] ? 0 : 1);
 
   RW_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
@@ -2849,7 +2517,7 @@ int32_t rwgpu_join_create(const rw_join_desc* d, rwgpu_join** out) {
       if (sd[s]->stored_rows_hint && s != h->uni_is) rows = std::max<uint64_t>(4096, sd[s]->stored_rows_hint);
       rc = join_grow_store(h, s, std::min<uint64_t>(rows, 0x40000000ull));
       if (rc != RW_OK) return rc;
-      RW_CUDA(h->side[s].pools.reserve((size_t)Q4_MAX_GRID * (JF_BLOCK / 32) * sizeof(uint2)));
+      RW_CUDA(h->side[s].pools.reserve((size_t)U_MAX_GRID * (JF_BLOCK / 32) * sizeof(uint2)));
       RW_CUDA(cudaMemsetAsync(h->side[s].pools.p, 0, h->side[s].pools.bytes, h->stream));
     }
   }
@@ -2863,9 +2531,6 @@ int32_t rwgpu_join_create(const rw_join_desc* d, rwgpu_join** out) {
     // overflow rows only; sized from the planner's cardinality hint (2 rows per expected key) so that a
     // stream of the expected size never pays a doubling (allocate + copy + free) in its data path
     rc = join_grow_store(h, s, std::max<uint64_t>(1024, std::min<uint64_t>(2 * hint, 0x40000000ull)));
-    if (rc != RW_OK) return rc;
-    RW_CUDA(h->side[s].pools.reserve((size_t)Q4_MAX_GRID * (JF_BLOCK / 32) * sizeof(uint2)));
-    RW_CUDA(cudaMemsetAsync(h->side[s].pools.p, 0, h->side[s].pools.bytes, h->stream));
     if (rc != RW_OK) return rc;
   }
   RW_CUDA(cudaStreamSynchronize(h->stream));

@@ -1,10 +1,9 @@
 // join_uni.cuh -- ONE hash table for both sides of a Key64 inner join (included by join.cu).
 //
-// The two-table inner kernel (join.cu) is bound by the NUMBER of random
-// 64-byte DRAM transactions per row -- probe line of the other side, own-side line read by the claiming
-// CAS, own-side write-back, and each 128-byte bucket-pair fetch counted twice.  Here a join key owns ONE
-// 64-byte bucket that carries the state of BOTH sides, so a row's probe and its own-side insert touch the
-// SAME line: one random read + one write-back per row, everything else is sequential.
+// The two-table inner kernels (join.cu) are bound by the NUMBER of random 64-byte DRAM transactions per
+// row -- probe line of the other side, own-side line read by the claiming CAS, own-side write-back.  Here a
+// join key owns ONE 64-byte bucket that carries the state of BOTH sides, so a row's probe and its own-side
+// insert touch the SAME line: one random read + one write-back per row, everything else is sequential.
 //
 //   bucket (64 B, linear probing bucket by bucket, load <= 0.5):
 //     +0   key                 J_EMPTY = free
@@ -32,6 +31,7 @@ namespace rw {
 
 #define U_NIL 0x7fffffffu
 #define U_XCHUNK 64  // extra-match output rows a warp reserves at a time
+#define U_MAX_GRID (RW_SMS * 8)  // blocks of JF_BLOCK threads of uni_hot_kernel; one id pool per warp and side
 
 // A side's log is a list of fixed-size SEGMENTS (2^22 records = 192 MiB each) reached through a small device table of
 // segment pointers: growing the log allocates one more segment and appends its pointer -- no copy of the existing
@@ -70,6 +70,17 @@ __device__ __forceinline__ uint8_t* useg_rec(uint8_t* const* segs, uint32_t id) 
 }
 __device__ __forceinline__ UniRec* urec(const UniDev& t, int side, uint32_t id) { return (UniRec*)useg_rec(t.log[side], id); }
 __device__ __forceinline__ uint64_t uhome(uint64_t key, uint64_t mask) { return mix64(key) & mask; }
+
+// a chunk whose row count lives on the device (e.g. the output of the exchange): clamp the capacity.
+// (uni_hot_kernel reports a count out of range; the kernels behind it treat it as no rows.)
+__device__ __forceinline__ int64_t chunk_rows(const DevChunk& ch) {
+  if (!ch.n_dev) return ch.n;
+  const int64_t n = *ch.n_dev;
+  return (n < 0 || n > ch.n) ? 0 : n;
+}
+__device__ __forceinline__ uint64_t shfl64m(unsigned mask, uint64_t v, int src) {
+  return (uint64_t)__shfl_sync(mask, (unsigned long long)v, src);
+}
 
 __global__ void uni_init_kernel(uint8_t* buckets, uint64_t from, uint64_t to) {
   for (uint64_t i = from + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < to; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -369,9 +380,10 @@ struct UniWork {
   uint8_t* mask;     // [(n + 7) / 8], one bit per input row, every byte written by the hot kernel
 };
 
-template <bool PROBE_ONLY, bool IS_ROW, int MINB>
-__global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, uint8_t* buckets, uint64_t cap, UniOwn own, PlainOut o, UniWork wk,
-                                                                  JoinStatus* st, uint64_t seq_base, int64_t out_base, uint32_t pool_chunk) {
+// 4 blocks of 256 threads per SM (64 registers): the kernel is bound by random DRAM transactions, not by occupancy
+template <bool PROBE_ONLY, bool IS_ROW>
+__global__ void __launch_bounds__(JF_BLOCK, 4) uni_hot_kernel(PlainChunk ch, uint8_t* buckets, uint64_t cap, UniOwn own, PlainOut o, UniWork wk,
+                                                               JoinStatus* st, uint64_t seq_base, int64_t out_base, uint32_t pool_chunk) {
   int64_t n_rows = ch.n;
   if (ch.n_dev) {
     const int64_t nd = *ch.n_dev;
@@ -678,7 +690,7 @@ __global__ void __launch_bounds__(JF_BLOCK, MINB) uni_hot_kernel(PlainChunk ch, 
 template <bool PROBE_ONLY>
 __device__ __forceinline__ void uni_deferred_body(const JoinPlanDev* __restrict__ p, const W8Plan& w, int S, const DevChunk& ch, const UniDev& t,
                                                   const JoinOutDev& o, const UniWork& wk, JoinStatus* st, uint64_t seq_base, int64_t out_base) {
-  const int64_t n_rows = chunk_rows(ch, st, false);
+  const int64_t n_rows = chunk_rows(ch);
   unsigned new_keys = 0;
   bool any_match = false, any_hole = false;
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
@@ -719,7 +731,7 @@ __device__ __forceinline__ bool uni_pk_equal(const JoinPlanDev* p, int S, const 
 // sentinel_mode: 0 = every delete row; 1 = all but the rows whose key is the EMPTY sentinel; 2 = only those, by ONE block
 __device__ __forceinline__ void uni_delete_body(const JoinPlanDev* __restrict__ p, int S, const DevChunk& ch, const UniDev& t, JoinStatus* st,
                                                 uint64_t seq_base, int sentinel_mode) {
-  const int64_t n_rows = chunk_rows(ch, st, false);
+  const int64_t n_rows = chunk_rows(ch);
   const uint64_t SEQ56 = (1ull << 56) - 1;
   unsigned int dead_log = 0;
   const int64_t r_first = sentinel_mode == 2 ? (int64_t)threadIdx.x : blockIdx.x * (int64_t)blockDim.x + threadIdx.x;

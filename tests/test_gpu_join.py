@@ -235,9 +235,10 @@ class StreamGen4(StreamGen):
 
 
 def test_inner_key64_four_columns_large_chunks(cuda, oracle):
-    """Inner join, one int64 key, 4 + 4 int64 columns = the quad-cooperative kernel (join_inner_q4_kernel):
-    chunks large enough for many warps and overflow-pool refills, hot keys (several matches per row),
-    deletes / updates, invisible rows, and the key that equals the table's EMPTY sentinel."""
+    """Inner join, one int64 key, 4 + 4 int64 columns = the unified table (uni_hot_kernel for plain chunks,
+    uni_slow_kernel for chunks with a visibility bitmap): chunks large enough for many warps and overflow-pool
+    refills, hot keys (several matches per row), deletes / updates, invisible rows, and the key that equals the
+    table's EMPTY sentinel."""
     types = [abi.T_INT64] * 4
     exs = make_pair(cuda, oracle, abi.JOIN_INNER, types, [0], [1], [1], [False])
     gen = StreamGen4(seed=5, key_range=600)
@@ -257,7 +258,7 @@ def test_inner_key64_four_columns_large_chunks(cuda, oracle):
 
 def test_join_push_device_counted_matches_exact_chunk(cuda):
     """rwgpu_join_push_device_counted: a chunk whose buffers are larger than its row count, the count living
-    on the device, gives the same output as the exact chunk (both through the quad-cooperative kernel)."""
+    on the device, gives the same output as the exact chunk (both through the quad-cooperative uni_hot_kernel)."""
     import torch
     from risingwave_b200 import device
     rng = np.random.default_rng(11)
@@ -319,17 +320,33 @@ def _set_seq(cuda, ex, seq):
     assert cuda.lib.rwgpu_join_debug_set_seq(ex._h, C.c_uint64(seq)) == 0
 
 
-@pytest.mark.parametrize("no_uni", [False, True], ids=["unified", "two_tables"])
+class StreamGen5(StreamGen4):
+    """StreamGen4 with a third payload column: rows are (key, pk, payload, payload2, payload3)."""
+
+    def new_row(self, side):
+        return super().new_row(side) + (int(self.rng.integers(0, 1 << 40)),)
+
+
+# Inner-join plan shapes and the kernels they select: the unified table (Key64, 4 eight-byte columns); two tables with
+# Key64 and 5 eight-byte columns (join_inner_w8p_kernel); two tables with an int32 column (join_inner_fused_kernel,
+# StreamGen's payload is below 50).  Both two-table kernels share join_inner_delete_kernel.
+DELETE_RULE_PLANS = {
+    "unified": (StreamGen4, [abi.T_INT64] * 4),
+    "two_tables_w8": (StreamGen5, [abi.T_INT64] * 5),
+    "two_tables_typed": (StreamGen4, [abi.T_INT64, abi.T_INT64, abi.T_INT32, abi.T_INT64]),
+}
+
+
+@pytest.mark.parametrize("plan", list(DELETE_RULE_PLANS))
 @pytest.mark.parametrize("seq0", [(1 << 31) - 700, (1 << 32) - 700, (1 << 33) + 5], ids=["2^31", "2^32", "2^33"])
-def test_delete_rule_across_arrival_counter_boundaries(cuda, oracle, monkeypatch, no_uni, seq0):
+def test_delete_rule_across_arrival_counter_boundaries(cuda, oracle, plan, seq0):
     """ADVICE r1 (high): the own-side delete picked its victim by a 32-bit wrap-aware age, so a live row inserted more
     than 2^31 arrivals ago could no longer be deleted.  Rows now carry a 64-bit arrival number; the counter is moved
     next to the boundaries through the test hook and a stream with deletes / same-pk re-inserts crosses them."""
-    if no_uni:
-        monkeypatch.setenv("RWGPU_NO_UNI", "1")
-    types = [abi.T_INT64] * 4
+    gen_cls, types = DELETE_RULE_PLANS[plan]
     exs = make_pair(cuda, oracle, abi.JOIN_INNER, types, [0], [1], [1], [False])
-    gen = StreamGen4(seed=21, key_range=40)
+    gen = gen_cls(seed=21, key_range=40)
+    more = (11,) * (len(types) - 4)  # payload columns of the hand-written rows beyond the fourth
     # rows stored long BEFORE the boundary ...
     _set_seq(cuda, exs[0], 5)
     first = [(s, gen.chunk(s, 400, p_delete=0.0, p_update=0.0, types=types)) for s in (0, 1)]
@@ -340,10 +357,10 @@ def test_delete_rule_across_arrival_counter_boundaries(cuda, oracle, monkeypatch
     for i in range(10):
         side = i % 2
         pushes.append((side, gen.chunk(side, 300, p_delete=0.45, p_update=0.25, types=types)))
-    pushes.append((0, StreamChunk.from_rows(types, [(abi.OP_INSERT, (3, 10 ** 9, 1, 2)), (abi.OP_DELETE, (3, 10 ** 9, 1, 2)),
-                                                    (abi.OP_INSERT, (3, 10 ** 9, 1, 2)), (abi.OP_DELETE, (3, 10 ** 9, 1, 2)),
-                                                    (abi.OP_INSERT, (3, 10 ** 9, 5, 6))])))
-    pushes.append((1, StreamChunk.from_rows(types, [(abi.OP_INSERT, (3, 10 ** 9 + 1, 7, 8))])))
+    pushes.append((0, StreamChunk.from_rows(types, [(abi.OP_INSERT, (3, 10 ** 9, 1, 2) + more), (abi.OP_DELETE, (3, 10 ** 9, 1, 2) + more),
+                                                    (abi.OP_INSERT, (3, 10 ** 9, 1, 2) + more), (abi.OP_DELETE, (3, 10 ** 9, 1, 2) + more),
+                                                    (abi.OP_INSERT, (3, 10 ** 9, 5, 6) + more)])))
+    pushes.append((1, StreamChunk.from_rows(types, [(abi.OP_INSERT, (3, 10 ** 9 + 1, 7, 8) + more)])))
     assert drive(exs, pushes) > 1000
 
 
