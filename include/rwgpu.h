@@ -257,7 +257,12 @@ void rwgpu_join_destroy(rwgpu_join* h);
  * until rwgpu_out_release(*out).  (RWGPU_NO_ALIAS=1 in the environment disables this.)            */
 int32_t rwgpu_join_push(rwgpu_join* h, int32_t side, const rw_chunk* chunk, rwgpu_out** out);
 /* DEVICE chunk; output left in HBM as one un-cut chunk `view` (device pointers, valid until the
- * next push on this handle).  *view.n_rows is read back (one 8-byte D2H).                    */
+ * next push on this handle).  *view.n_rows is read back (one 8-byte D2H).
+ * ALIASING: when the output is positional (output row r belongs to input row r) the view's columns
+ * that are plain copies of `chunk`'s columns may point into `chunk`'s own device buffers instead of
+ * a copy.  Keep `chunk`'s buffers alive and unmodified for as long as the view is used: until the
+ * next push on this handle (for the _async / collect pair below: until the second _async after
+ * the push).  A chunk with a device-resident row count is never aliased.                      */
 int32_t rwgpu_join_push_device(rwgpu_join* h, int32_t side, const rw_chunk* chunk, rw_chunk* view,
                                void* cuda_stream);
 /* same, for a chunk whose row count is produced ON THE DEVICE by earlier work of `cuda_stream` (the
@@ -270,7 +275,8 @@ int32_t rwgpu_join_push_device_counted(rwgpu_join* h, int32_t side, const rw_chu
  * `_async` only ENQUEUES the push on `cuda_stream` (n_rows_dev may be NULL) and returns; `rwgpu_join_collect` waits
  * for the OLDEST outstanding push and returns its output like the synchronous call.  Rules:
  *  - at most two pushes outstanding (two output sets); a view stays valid until the second `_async` after its own;
- *  - `chunk`'s DEVICE buffers (and *n_rows_dev) stay valid and unmodified until the push is collected;
+ *  - `chunk`'s DEVICE buffers (and *n_rows_dev) stay valid and unmodified until the push is collected, and as long as
+ *    its view is used when the view aliases them (see rwgpu_join_push_device);
  *  - pushes of DIFFERENT sides are never outstanding together (RW_ERR_INVALID): a side's probe reads the other side's
  *    state, and the collect step may have to re-run that probe when the output area was too small;
  *  - errors of the push (RW_ERR_INCONSISTENT ...) are reported by its collect;

@@ -1506,6 +1506,9 @@ struct JoinPending {
   cudaStream_t st = nullptr;
   int64_t out_base = 0;
   bool plain = true, counted = false, sync_done = false;
+  // the hot kernel leaves the update-side output columns unwritten: the view points at ch's columns, or collect fills
+  // them from there (uni_finish)
+  bool alias_u = false;
   uint32_t pool_chunk = 0;
   uint64_t seq_base = 0, ids_before = 0, keys_before = 0;
   unsigned long long tag = 0;
@@ -1932,7 +1935,7 @@ static int uni_launch_main(rwgpu_join* h, const JoinPending& pd, bool probe_only
     po.ops = od.ops;
     po.vis = od.vis;
     for (int c = 0; c < 4; c++) {
-      po.ucol[c] = (c < w.n_u && w.u_out[c] >= 0) ? (unsigned long long*)od.col[w.u_out[c]] : nullptr;
+      po.ucol[c] = (!pd.alias_u && c < w.n_u && w.u_out[c] >= 0) ? (unsigned long long*)od.col[w.u_out[c]] : nullptr;
       po.mcol[c] = (c < w.n_m && w.m_out[c] >= 0) ? (unsigned long long*)od.col[w.m_out[c]] : nullptr;
     }
     po.capacity = od.capacity;
@@ -1979,10 +1982,13 @@ static int join_plain_chunk(DevChunk* ch, bool device_count, cudaStream_t st, bo
 
 // LAUNCH half of a push: main kernel + delete kernel (which publishes the status block into the output set's pinned
 // slot) are enqueued on `st`; nothing is waited for.  The output goes to the CURRENT output set (h->cur).
+// `alias_ok`: the caller hands the output over as a device view, which may point into the chunk's own columns.  A
+// plain chunk with a host-known row count then skips the update-side column stores in uni_hot_kernel.  A counted chunk
+// does not: its buffer (an exchange's receive buffer) is rewritten while the view may still be read.
 static double uni_now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 static const bool uni_trace = getenv("RWGPU_TRACE") != nullptr;  // host-side timeline on stderr (debugging only)
 
-static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t st, int64_t out_base, JoinPending* pd) {
+static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t st, int64_t out_base, bool alias_ok, JoinPending* pd) {
   const double tr0 = uni_trace ? uni_now_ms() : 0.0;
   DevChunk ch = ch_in;
   bool plain_cols;
@@ -2020,6 +2026,7 @@ static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t
   pd->set = h->cur;
   pd->plain = plain_cols;
   pd->counted = counted;
+  pd->alias_u = alias_ok && plain_cols && !counted && out_base == 0 && h->var_in[S].empty();
   pd->grid = grid;
   pd->pool_chunk = pool_chunk;
   pd->seq_base = h->seq;
@@ -2041,8 +2048,9 @@ static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t
 }
 
 // COLLECT half: wait for the push, read its status, redo the (state-free) emission if the extra-match area was too
-// small, settle the host's bookkeeping.  h->cur must be pd.set.
-static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, unsigned long long* null_mask) {
+// small, settle the host's bookkeeping.  h->cur must be pd.set.  *aliased (if given): the view's update-side columns
+// are the input chunk's (join_fill_view).
+static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, unsigned long long* null_mask, bool* aliased = nullptr) {
   cudaStream_t st = pd.st;
   JoinStatus* ds = h->status.as<JoinStatus>();
   JoinStatus* slot = (JoinStatus*)(h->status_host.as<uint8_t>() + 512 * pd.set);
@@ -2104,6 +2112,17 @@ static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, u
   *null_mask = h->call_null_mask;
   h->os().valid_dirty |= hs.null_mask & ((1ull << 63) - 1);
   if (hs.n_del) h->call_had_deletes = true;
+  // pd.alias_u: the view may use the input's columns only while output row r is input row r and nothing on the device
+  // reads the output columns first (the no-op pass does).  Otherwise rows [0, n) are filled from the input here; the
+  // deferred rows already hold the same values.  A PROBE_ONLY redo skips the columns as well and relies on this fill.
+  const bool alias = pd.alias_u && !redone && hs.out_rows == 0 && !h->call_had_deletes;
+  if (pd.alias_u && !alias && *out_rows > 0) {
+    const W8Plan& w = h->w8[pd.S];
+    for (int c = 0; c < w.n_u; c++)
+      if (w.u_out[c] >= 0)
+        RW_CUDA(cudaMemcpyAsync(h->os().out_col[w.u_out[c]].p, pd.ch.cols[c].data, (size_t)pd.ch.n * 8, cudaMemcpyDeviceToDevice, st));
+  }
+  if (aliased) *aliased = alias;
   if (uni_trace)
     fprintf(stderr, "  [uni_finish S=%d set=%d] wait %.3f ms, rest %.3f ms (redo %d, extras %llu, n_del %llu, out %lld)\n", pd.S, pd.set, tr1 - tr0,
             uni_now_ms() - tr1, (int)redone, (unsigned long long)hs.out_rows,
@@ -2112,25 +2131,28 @@ static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, u
 }
 
 static int join_push_dev_uni(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t st, int64_t out_base, int64_t* out_rows,
-                             unsigned long long* null_mask) {
+                             unsigned long long* null_mask, bool* aliased) {
   if (h->n_pending) return fail(RW_ERR_INVALID, "collect the outstanding asynchronous pushes first");
   JoinPending pd;
-  int rc = uni_enqueue(h, S, ch_in, st, out_base, &pd);
+  int rc = uni_enqueue(h, S, ch_in, st, out_base, aliased != nullptr, &pd);
   if (rc != RW_OK) return rc;
-  return uni_finish(h, pd, out_rows, null_mask);
+  return uni_finish(h, pd, out_rows, null_mask, aliased);
 }
 
 // one push of a device-resident chunk; on return the output sits in the device output buffers.
 // *null_mask: bit k = output column k holds NULLs, bit 63 = some rows are invisible.
 // `out_base` rows of the device output buffers are already occupied by earlier sub-batches of the
 // same API call (the caller zeroed status.out_rows / null_mask before the first one).
+// `aliased` (device views only; nullptr = every output column is written): set when the update-side output columns
+// were left in ch_in's columns (uni_finish).
 static int join_push_dev(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t st, int64_t out_base, int64_t* out_rows,
-                         unsigned long long* null_mask) {
+                         unsigned long long* null_mask, bool* aliased = nullptr) {
   *out_rows = 0;
+  if (aliased) *aliased = false;
   DevChunk ch = ch_in;
   if (ch.n <= 0) return RW_OK;
   if (ch.n >= (1ll << 31)) return fail(RW_ERR_INVALID, "chunk too large");
-  if (h->uni) return join_push_dev_uni(h, S, ch_in, st, out_base, out_rows, null_mask);
+  if (h->uni) return join_push_dev_uni(h, S, ch_in, st, out_base, out_rows, null_mask, aliased);
   // no two-table kernel reads a device-resident row count: it is read back first
   bool plain_cols;
   int rc = join_plain_chunk(&ch, false, st, &plain_cols);
@@ -2663,8 +2685,10 @@ static int join_post_process(rwgpu_join* h, int64_t n, unsigned long long* nullm
   return RW_OK;
 }
 
-// device view of the current output set's first n rows (bitmaps are packed on `st` where NULLs / holes exist)
-static int join_fill_view(rwgpu_join* h, int64_t n, unsigned long long nullm, rw_chunk* view, cudaStream_t st) {
+// device view of the current output set's first n rows (bitmaps are packed on `st` where NULLs / holes exist).
+// alias_in: the push of side S left its update-side output columns in this chunk (join_push_dev); the view points there.
+static int join_fill_view(rwgpu_join* h, int64_t n, unsigned long long nullm, rw_chunk* view, cudaStream_t st, const DevChunk* alias_in = nullptr,
+                          int S = 0) {
   std::vector<rw_column>& cols = h->dev_view_cols[h->cur];
   cols.resize(h->out_types.size());
   for (size_t k = 0; k < h->out_types.size(); k++) {
@@ -2688,6 +2712,9 @@ static int join_fill_view(rwgpu_join* h, int64_t n, unsigned long long nullm, rw
       col.validity = h->os().out_bits[k].as<uint64_t>();
     }
   }
+  if (alias_in)
+    for (int c = 0; c < h->w8[S].n_u; c++)
+      if (h->w8[S].u_out[c] >= 0) cols[(size_t)h->w8[S].u_out[c]].data = alias_in->cols[c].data;
   view->n_rows = n;
   view->n_cols = (int32_t)h->out_types.size();
   view->reserved = 0;
@@ -2719,11 +2746,12 @@ int32_t rwgpu_join_push_device_counted(rwgpu_join* h, int32_t side, const rw_chu
   if (rc != RW_OK) return rc;
   rc = var_intern_device_chunk(h, side, c, &ch, st);
   if (rc != RW_OK) return rc;
-  rc = join_push_dev(h, side, ch, st, 0, &n, &nullm);
+  bool aliased = false;
+  rc = join_push_dev(h, side, ch, st, 0, &n, &nullm, &aliased);
   if (rc != RW_OK) return rc;
   rc = join_post_process(h, n, &nullm, st);
   if (rc != RW_OK) return rc;
-  return join_fill_view(h, n, nullm, view, st);
+  return join_fill_view(h, n, nullm, view, st, aliased ? &ch : nullptr, side);
 }
 
 // LAUNCH half (see rwgpu.h).  Unified-table handles really only enqueue; other plan shapes run the push to
@@ -2747,7 +2775,7 @@ int32_t rwgpu_join_push_device_async(rwgpu_join* h, int32_t side, const rw_chunk
   rc = var_intern_device_chunk(h, side, c, &ch, st);
   if (rc != RW_OK) return rc;
   if (h->uni && ch.n > 0 && ch.n < (1ll << 31) && h->var_in[side].empty()) {
-    rc = uni_enqueue(h, side, ch, st, 0, &pd);
+    rc = uni_enqueue(h, side, ch, st, 0, true, &pd);
     if (rc != RW_OK) return rc;
   } else {
     pd.S = side;
@@ -2773,17 +2801,18 @@ int32_t rwgpu_join_collect(rwgpu_join* h, rw_chunk* view, void* cuda_stream) {
   h->cur = pd.set;
   int64_t n = pd.rows;
   unsigned long long nullm = pd.nullm;
+  bool aliased = false;
   if (!pd.sync_done) {
     h->call_null_mask = 0;
     h->call_had_deletes = false;
-    int rc = uni_finish(h, pd, &n, &nullm);
+    int rc = uni_finish(h, pd, &n, &nullm, &aliased);
     if (rc != RW_OK) return rc;
     const double tp0 = uni_trace ? uni_now_ms() : 0.0;
     rc = join_post_process(h, n, &nullm, pd.st);
     if (rc != RW_OK) return rc;
     if (uni_trace) fprintf(stderr, "  [collect] post-process (no-op elimination: %d) %.3f ms\n", (int)h->call_had_deletes, uni_now_ms() - tp0);
   }
-  int rc = join_fill_view(h, n, nullm, view, cuda_stream ? (cudaStream_t)cuda_stream : pd.st);
+  int rc = join_fill_view(h, n, nullm, view, cuda_stream ? (cudaStream_t)cuda_stream : pd.st, aliased ? &pd.ch : nullptr, pd.S);
   // the next synchronous push must not land in the set a still-outstanding push writes to
   if (h->n_pending) h->cur = h->pending[h->n_pending - 1].set;
   return rc;
@@ -3117,7 +3146,7 @@ int32_t rwgpu_join_push_async(rwgpu_join* h, int32_t side, const rw_chunk* c) {
   int rc = join_begin_call(h, h->stream);
   if (rc != RW_OK) { hp.active = false; return rc; }
   RW_CUDA(cudaStreamWaitEvent(h->stream, h->ev_up2[set], 0));
-  rc = uni_enqueue(h, side, ch, h->stream, 0, &pd);
+  rc = uni_enqueue(h, side, ch, h->stream, 0, false, &pd);
   if (rc != RW_OK) { hp.active = false; return rc; }
   // ---- output block + the copy-out of the positional rows
   auto o = new rwgpu_out();

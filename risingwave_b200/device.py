@@ -6,6 +6,7 @@ hash-shuffle path (exchange.py).  PyTorch is plumbing here: allocation, streams,
 """
 from __future__ import annotations
 
+import collections
 import ctypes as C
 from typing import List, Optional, Sequence
 
@@ -57,10 +58,12 @@ class DeviceChunk:
 class DeviceView:
     """Device pointers returned by a `*_device` call (valid until the next call on that handle)."""
 
-    def __init__(self, view: abi.RwChunk, stream: Optional[torch.cuda.Stream] = None):
+    def __init__(self, view: abi.RwChunk, stream: Optional[torch.cuda.Stream] = None, chunk: Optional[DeviceChunk] = None):
         # the library may still be packing bitmaps on `stream` when the call returns: readers below wait for it
         self._stream = stream
         self._synced = False
+        # a join view's update-side columns may point into the pushed chunk's tensors (rwgpu.h): they live as long as the view
+        self._chunk = chunk
         self.n_rows = int(view.n_rows)
         self.n_cols = int(view.n_cols)
         self.ops_ptr = view.ops
@@ -243,22 +246,27 @@ def join_push_device(executor, side: int, chunk: DeviceChunk, stream: Optional[t
     else:
         _check(_lib().rwgpu_join_push_device_counted(executor._h, side, C.byref(ch), C.c_void_p(n_rows_dev), C.byref(view),
                                                      _stream_ptr(stream)))
-    return DeviceView(view, stream)
+    return DeviceView(view, stream, chunk)
 
 
 def join_push_device_async(executor, side: int, chunk: DeviceChunk, stream: Optional[torch.cuda.Stream] = None,
                            n_rows_dev: Optional[int] = None):
-    """LAUNCH half of a push (nothing is waited for); the chunk's tensors must stay alive until `join_collect`"""
+    """LAUNCH half of a push (nothing is waited for); the chunk is kept alive until `join_collect` hands it to the view"""
     ch, keep = chunk.to_abi()
     _check(_lib().rwgpu_join_push_device_async(executor._h, side, C.byref(ch), C.c_void_p(n_rows_dev) if n_rows_dev else None,
                                                _stream_ptr(stream)))
+    if not hasattr(executor, "_pushed_chunks"):
+        executor._pushed_chunks = collections.deque()
+    executor._pushed_chunks.append(chunk)
 
 
 def join_collect(executor, stream: Optional[torch.cuda.Stream] = None) -> DeviceView:
     """COLLECT half: wait for the oldest outstanding push; -> its output (device pointers)"""
     view = abi.RwChunk()
+    pushed = getattr(executor, "_pushed_chunks", None)
+    chunk = pushed.popleft() if pushed else None  # (a collect that fails still takes the oldest push off the handle)
     _check(_lib().rwgpu_join_collect(executor._h, C.byref(view), _stream_ptr(stream)))
-    return DeviceView(view, stream)
+    return DeviceView(view, stream, chunk)
 
 
 def profile(executor, kind: str, enable: bool):
