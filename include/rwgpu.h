@@ -254,7 +254,7 @@ void rwgpu_join_destroy(rwgpu_join* h);
  * ALIASING: for an inner join whose output is positional (output row r belongs to input row r), the
  * output columns that are plain copies of `chunk`'s columns are NOT shipped back over PCIe: the output
  * chunk views point into `chunk`'s own column buffers.  Keep `chunk`'s buffers alive and unmodified
- * until rwgpu_out_release(*out).  (RWGPU_NO_ALIAS=1 in the environment disables this.)            */
+ * until rwgpu_out_release(*out).                                                                   */
 int32_t rwgpu_join_push(rwgpu_join* h, int32_t side, const rw_chunk* chunk, rwgpu_out** out);
 /* DEVICE chunk; output left in HBM as one un-cut chunk `view` (device pointers, valid until the
  * next push on this handle).  *view.n_rows is read back (one 8-byte D2H).

@@ -33,7 +33,6 @@
 //     key's rows in input order -- state of different keys is disjoint, so this is exactly the
 //     reference's sequential semantics with the parallelism taken across keys.
 #include <algorithm>
-#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <memory>
@@ -1569,20 +1568,17 @@ struct rwgpu_join {
   } oset[2];
   int cur = 0;
   OutSet& os() { return oset[cur]; }
-  // host staging
-  DevBuf up;
-  PinnedBuf up_host;
-  // launch / collect split for HOST chunks (rwgpu_join_push_async / rwgpu_join_collect_out): per output set, the device
-  // staging of the input, the pinned output block and what collect still has to copy
+  // launch / collect split for HOST chunks (rwgpu_join_push_async / rwgpu_join_collect_out): per output set, the pinned
+  // output block and what collect still has to copy
   struct HostPending {
-    bool active = false, sync_done = false;
-    rwgpu_out* out = nullptr;      // sync_done: the finished result; else the block the copies land in
-    rw_chunk in;                   // the caller's chunk (its buffers stay valid until collect: rwgpu.h)
-    std::vector<rw_column> in_cols;
+    bool active = false;
+    rwgpu_out* out = nullptr;      // a push completed at launch: the finished result; else the block the copies land in
+    std::vector<rw_column> in_cols;  // the caller's columns (their buffers stay valid until collect: rwgpu.h)
     std::vector<int> alias_src;
     int64_t n = 0, host_cap = 0;
-    bool alias_ok = false;
   } hpend[2];
+  // host-chunk staging, per output set (device + pinned): a synchronous push uses the current set's, an asynchronous one
+  // the set its output goes to
   DevBuf up2[2];
   PinnedBuf up2_host[2];
   cudaEvent_t ev_up2[2] = {nullptr, nullptr};
@@ -1605,6 +1601,7 @@ struct rwgpu_join {
     for (auto e : ev_h2d) if (e) cudaEventDestroy(e);
     for (auto e : ev_main) if (e) cudaEventDestroy(e);
     for (auto e : pend_ev) if (e) cudaEventDestroy(e);
+    for (auto e : ev_up2) if (e) cudaEventDestroy(e);
     if (order_ev) cudaEventDestroy(order_ev);
     if (s_h2d) cudaStreamDestroy(s_h2d);
     if (s_d2h) cudaStreamDestroy(s_d2h);
@@ -1985,11 +1982,7 @@ static int join_plain_chunk(DevChunk* ch, bool device_count, cudaStream_t st, bo
 // `alias_ok`: the caller hands the output over as a device view, which may point into the chunk's own columns.  A
 // plain chunk with a host-known row count then skips the update-side column stores in uni_hot_kernel.  A counted chunk
 // does not: its buffer (an exchange's receive buffer) is rewritten while the view may still be read.
-static double uni_now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-static const bool uni_trace = getenv("RWGPU_TRACE") != nullptr;  // host-side timeline on stderr (debugging only)
-
 static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t st, int64_t out_base, bool alias_ok, JoinPending* pd) {
-  const double tr0 = uni_trace ? uni_now_ms() : 0.0;
   DevChunk ch = ch_in;
   bool plain_cols;
   int rc = join_plain_chunk(&ch, true, st, &plain_cols);
@@ -2018,7 +2011,6 @@ static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t
   }
   rc = join_order(h, st);
   if (rc != RW_OK) return rc;
-  const double tr1 = uni_trace ? uni_now_ms() : 0.0;
   pd->S = S;
   pd->ch = ch;
   pd->st = st;
@@ -2040,10 +2032,6 @@ static int uni_enqueue(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream_t
   if (rc != RW_OK) return rc;
   if (!h->pend_ev[pd->set]) RW_CUDA(cudaEventCreateWithFlags(&h->pend_ev[pd->set], cudaEventDisableTiming));
   RW_CUDA(cudaEventRecord(h->pend_ev[pd->set], st));
-  if (uni_trace)
-    fprintf(stderr, "  [uni_enqueue S=%d n=%lld set=%d] grow/ensure %.3f ms, launch %.3f ms (log segs %zu/%zu, cap %llu keys<=%llu)\n", S, (long long)n,
-            pd->set, tr1 - tr0, uni_now_ms() - tr1, h->side[0].log.segs.size(), h->side[1].log.segs.size(), (unsigned long long)h->uni_cap,
-            (unsigned long long)h->uni_keys);
   return RW_OK;
 }
 
@@ -2055,9 +2043,7 @@ static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, u
   JoinStatus* ds = h->status.as<JoinStatus>();
   JoinStatus* slot = (JoinStatus*)(h->status_host.as<uint8_t>() + 512 * pd.set);
   JoinStatus hs;
-  const double tr0 = uni_trace ? uni_now_ms() : 0.0;
   RW_CUDA(cudaEventSynchronize(h->pend_ev[pd.set]));
-  const double tr1 = uni_trace ? uni_now_ms() : 0.0;
   int rc;
   if (*(volatile unsigned long long*)(slot + 1) != pd.tag) return fail(RW_ERR_CUDA, "join status block was not published");
   memcpy(&hs, slot, sizeof(JoinStatus));
@@ -2123,10 +2109,6 @@ static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, u
         RW_CUDA(cudaMemcpyAsync(h->os().out_col[w.u_out[c]].p, pd.ch.cols[c].data, (size_t)pd.ch.n * 8, cudaMemcpyDeviceToDevice, st));
   }
   if (aliased) *aliased = alias;
-  if (uni_trace)
-    fprintf(stderr, "  [uni_finish S=%d set=%d] wait %.3f ms, rest %.3f ms (redo %d, extras %llu, n_del %llu, out %lld)\n", pd.S, pd.set, tr1 - tr0,
-            uni_now_ms() - tr1, (int)redone, (unsigned long long)hs.out_rows,
-            (unsigned long long)hs.n_del, (long long)*out_rows);
   return RW_OK;
 }
 
@@ -2160,18 +2142,10 @@ static int join_push_dev(rwgpu_join* h, int S, const DevChunk& ch_in, cudaStream
   if (ch.n == 0) return RW_OK;  // the device-resident count was zero
   const int64_t n = ch.n;
   JoinSideHost& own = h->side[S];
-  static const bool trace = getenv("RWGPU_TRACE") != nullptr;
-  auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  const double tt0 = now();
-  const uint64_t cap0 = own.slot_cap, rcap0 = own.row_cap;
   rc = join_grow_store(h, S, own.n_rows + (uint64_t)n);
   if (rc != RW_OK) return rc;
   rc = join_grow_slots(h, S, own.keys_upper + (uint64_t)n);
   if (rc != RW_OK) return rc;
-  if (trace)
-    fprintf(stderr, "  [push_dev S=%d n=%lld] grow %.3f ms (slot_cap %llu->%llu, row_cap %llu->%llu, n_rows %llu keys %llu)\n", S, (long long)n,
-            now() - tt0, (unsigned long long)cap0, (unsigned long long)own.slot_cap, (unsigned long long)rcap0,
-            (unsigned long long)own.row_cap, (unsigned long long)own.n_rows, (unsigned long long)own.keys_upper);
   JoinStatus* ds = h->status.as<JoinStatus>();
   const JoinPlanDev* pd = h->plan_dev.as<JoinPlanDev>();
   // n_store / n_del are zero here: every status read-back resets them (join_status_publish)
@@ -2807,10 +2781,8 @@ int32_t rwgpu_join_collect(rwgpu_join* h, rw_chunk* view, void* cuda_stream) {
     h->call_had_deletes = false;
     int rc = uni_finish(h, pd, &n, &nullm, &aliased);
     if (rc != RW_OK) return rc;
-    const double tp0 = uni_trace ? uni_now_ms() : 0.0;
     rc = join_post_process(h, n, &nullm, pd.st);
     if (rc != RW_OK) return rc;
-    if (uni_trace) fprintf(stderr, "  [collect] post-process (no-op elimination: %d) %.3f ms\n", (int)h->call_had_deletes, uni_now_ms() - tp0);
   }
   int rc = join_fill_view(h, n, nullm, view, cuda_stream ? (cudaStream_t)cuda_stream : pd.st, aliased ? &pd.ch : nullptr, pd.S);
   // the next synchronous push must not land in the set a still-outstanding push writes to
@@ -2818,238 +2790,294 @@ int32_t rwgpu_join_collect(rwgpu_join* h, rw_chunk* view, void* cuda_stream) {
   return rc;
 }
 
-// HOST chunk.  Large chunks are cut into sub-batches (multiples of 64 rows, so bitmap words split
-// cleanly) that flow through three streams: H2D of sub-batch j+1 overlaps the kernels of j and the
-// D2H of j-1.  Sub-batches are ordinary consecutive pushes, so the operator semantics are unchanged;
-// their outputs land back to back in one device buffer and one pinned host block.
-int32_t rwgpu_join_push(rwgpu_join* h, int32_t side, const rw_chunk* c, rwgpu_out** out) {
-  if (!h || !c || !out) return fail(RW_ERR_INVALID, "null");
-  if (side != 0 && side != 1) return fail(RW_ERR_INVALID, "side");
-  if (c->n_cols != h->side[side].n_cols) return fail(RW_ERR_INVALID, "chunk schema mismatch");
-  for (int k = 0; k < c->n_cols; k++)
-    if (c->columns[k].type != h->side[side].types[k]) return fail(RW_ERR_INVALID, "chunk column type mismatch");
-  if (h->n_pending) return fail(RW_ERR_INVALID, "collect the outstanding asynchronous pushes first");
-  const int64_t n = c->n_rows;
-  static const bool trace = getenv("RWGPU_TRACE") != nullptr;
-  auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  const double t0 = now();
-  if (!h->s_h2d) {
-    RW_CUDA(cudaStreamCreateWithFlags(&h->s_h2d, cudaStreamNonBlocking));
-    RW_CUDA(cudaStreamCreateWithFlags(&h->s_d2h, cudaStreamNonBlocking));
-    for (int i = 0; i < 8; i++) {
-      RW_CUDA(cudaEventCreateWithFlags(&h->ev_h2d[i], cudaEventDisableTiming));
-      RW_CUDA(cudaEventCreateWithFlags(&h->ev_main[i], cudaEventDisableTiming));
-    }
-  }
-  // each sub-batch costs one status read-back: keep them >= 32K rows
-  const int J = n >= (1 << 19) ? 8 : (n >= (1 << 17) ? 4 : (n >= (1 << 16) ? 2 : 1));
-  int64_t sub = (n + J - 1) / J;
-  sub = (sub + 63) / 64 * 64;
-  // device staging: [ops | vis words | per column: data, valid words], regions sized for the whole chunk
-  const size_t nw = (size_t)((n + 63) / 64) * 8;
-  size_t off = 0;
-  auto region = [&](size_t bytes) { size_t o = align_up_j(off, 256); off = o + bytes; return o; };
-  const size_t o_ops = region((size_t)n), o_vis = region(nw);
-  size_t o_data[RW_MAX_COLS], o_valid[RW_MAX_COLS], o_voff[RW_MAX_COLS], o_vbytes[RW_MAX_COLS];
-  uint64_t var_bytes_in = 0;  // bytes of the chunk's varlen columns (interned into the side's heap below)
-  for (int k = 0; k < c->n_cols; k++) {
-    o_data[k] = region((size_t)n * type_width(c->columns[k].type));  // (varlen: the 8-byte handles)
-    o_valid[k] = region(nw);
-    o_voff[k] = o_vbytes[k] = 0;
-    if (type_is_varlen(c->columns[k].type)) {
-      if (n && !c->columns[k].offsets) return fail(RW_ERR_INVALID, "varlen column without offsets");
-      const size_t vb = n ? (size_t)(c->columns[k].offsets[n] - c->columns[k].offsets[0]) : 0;
-      o_voff[k] = region((size_t)(n + 1) * 4);
-      o_vbytes[k] = region(vb + 16);
-      var_bytes_in += vb + 8ull * (uint64_t)n;
-    }
-  }
-  if (var_bytes_in) {
-    int rcv = var_ensure_heap(h, side, var_bytes_in);
-    if (rcv != RW_OK) return rcv;
-    h->var_upper[side] += var_bytes_in;
-  }
-  RW_CUDA(h->up.reserve(off + 256));
-  RW_CUDA(h->up_host.reserve(off + 256));
-  uint8_t* hp = h->up_host.as<uint8_t>();
-  uint8_t* dp = h->up.as<uint8_t>();
-  // a caller buffer that is already pinned is copied straight from user memory; pageable small
-  // pieces go through the pinned staging block (one memcpy), pageable large ones directly
-  auto is_pinned = [](const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeHost;
-  };
-  auto h2d = [&](size_t dst_off, const void* src, size_t bytes, bool pinned) {
-    if (!bytes) return;
-    if (pinned || bytes >= (1u << 20)) cudaMemcpyAsync(dp + dst_off, src, bytes, cudaMemcpyHostToDevice, h->s_h2d);
-    else { memcpy(hp + dst_off, src, bytes); cudaMemcpyAsync(dp + dst_off, hp + dst_off, bytes, cudaMemcpyHostToDevice, h->s_h2d); }
-  };
-  RW_CUDA(cudaStreamSynchronize(h->s_d2h));  // previous call's copies are long done; cheap guard for buffer reuse
-  bool pin_ops = n ? is_pinned(c->ops) : false, pin_col[RW_MAX_COLS];
-  for (int k = 0; k < c->n_cols; k++) pin_col[k] = n ? is_pinned(c->columns[k].data) : false;
-  // enqueue every sub-batch's H2D up front
-  int n_sub = 0;
-  for (int64_t lo = 0; lo < n; lo += sub, n_sub++) {
-    const int64_t m = std::min<int64_t>(sub, n - lo);
-    const size_t wlo = (size_t)(lo / 64) * 8, wn = (size_t)((m + 63) / 64) * 8;
-    h2d(o_ops + (size_t)lo, c->ops + lo, (size_t)m, pin_ops);
-    if (c->visibility) h2d(o_vis + wlo, (const uint8_t*)c->visibility + wlo, wn, false);
-    for (int k = 0; k < c->n_cols; k++) {
-      const int w = type_width(c->columns[k].type);
-      if (type_is_varlen(c->columns[k].type)) {  // offsets lo .. lo+m and the bytes they span
-        const uint32_t* of = c->columns[k].offsets;
-        h2d(o_voff[k] + (size_t)lo * 4, of + lo, (size_t)(m + 1) * 4, false);
-        h2d(o_vbytes[k] + (size_t)(of[lo] - of[0]), (const uint8_t*)c->columns[k].data + of[lo], (size_t)(of[lo + m] - of[lo]), pin_col[k]);
-      } else {
-        h2d(o_data[k] + (size_t)lo * w, (const uint8_t*)c->columns[k].data + (size_t)lo * w, (size_t)m * w, pin_col[k]);
-      }
-      if (c->columns[k].validity) h2d(o_valid[k] + wlo, (const uint8_t*)c->columns[k].validity + wlo, wn, false);
-    }
-    RW_CUDA(cudaEventRecord(h->ev_h2d[n_sub], h->s_h2d));
-  }
-  RW_CUDA(cudaGetLastError());
-  const double t1 = now();
-  int rc = join_begin_call(h, h->stream);
-  if (rc != RW_OK) return rc;
-  auto o = new rwgpu_out();
-  std::unique_ptr<rwgpu_out> guard(o);
-  o->chunk_size = h->chunk_size;
-  // pinned host block laid out for `host_cap` rows; re-laid (host copy of the prefix) if outputs exceed it
-  int64_t host_cap = std::max<int64_t>(2 * n, 1024);
-  if (!o->layout(host_cap, h->out_types, ~0ull >> 1, true, h->pool)) return fail(RW_ERR_OOM, "pinned output block");
-  // Positional inner-join output (row r of the output = input row r): the update side's output columns are
-  // byte-for-byte the caller's input columns, which already sit in host memory -- they are not copied back
-  // over PCIe; the output chunk views alias the input buffers instead (contract in rwgpu.h).
-  static const bool no_alias = getenv("RWGPU_NO_ALIAS") != nullptr;
-  bool alias_ok = !no_alias && h->fast_inner && h->w8_ok[side] && !c->visibility && n > 0;
-  for (int k = 0; k < c->n_cols && alias_ok; k++) alias_ok = c->columns[k].validity == nullptr;
-  std::vector<int> alias_src(h->out_types.size(), -1);
-  if (alias_ok)
-    for (int k = 0; k < c->n_cols; k++)
-      if (h->w8[side].u_out[k] >= 0 && !type_is_varlen(c->columns[k].type)) alias_src[(size_t)h->w8[side].u_out[k]] = k;
-  bool aligned = true;  // every sub-batch produced exactly its positional rows (no extras, no empty result)
-  int64_t total = 0;
-  unsigned long long nullm = 0;
-  int js = 0;
-  const double t2 = now();
-  for (int64_t lo = 0; lo < n; lo += sub, js++) {
-    const int64_t m = std::min<int64_t>(sub, n - lo);
-    DevChunk ch;
-    memset(&ch, 0, sizeof(ch));
-    ch.n = m;
-    ch.n_cols = c->n_cols;
-    ch.ops = dp + o_ops + lo;
-    ch.vis_bits = c->visibility ? (const uint64_t*)(dp + o_vis + (size_t)(lo / 64) * 8) : nullptr;
-    for (int k = 0; k < c->n_cols; k++) {
-      const int w = type_width(c->columns[k].type);
-      ch.cols[k].type = c->columns[k].type;
-      ch.cols[k].width = w;
-      ch.cols[k].data = dp + o_data[k] + (size_t)lo * w;
-      ch.cols[k].valid_bits = c->columns[k].validity ? (const uint64_t*)(dp + o_valid[k] + (size_t)(lo / 64) * 8) : nullptr;
-    }
-    double ta = 0, tb = 0;
-    if (trace) { ta = now(); cudaEventSynchronize(h->ev_h2d[js]); tb = now(); }
-    RW_CUDA(cudaStreamWaitEvent(h->stream, h->ev_h2d[js], 0));
-    for (int k : h->var_in[side]) {  // bytes -> the side's heap, the column becomes a column of handles
-      rc = var_intern(h, side, dp + o_vbytes[k] - c->columns[k].offsets[0], (const uint32_t*)(dp + o_voff[k]) + lo, ch.ops, ch.vis_bits,
-                      ch.cols[k].valid_bits, m, (uint64_t*)(dp + o_data[k]) + lo, h->stream);
-      if (rc != RW_OK) { cudaStreamSynchronize(h->s_d2h); return rc; }
-    }
-    int64_t rows = 0;
-    rc = join_push_dev(h, side, ch, h->stream, total, &rows, &nullm);
-    if (trace) fprintf(stderr, "   sub %d: wait-h2d %.3f  push_dev %.3f ms\n", js, tb - ta, now() - tb);
-    if (rc != RW_OK) { cudaStreamSynchronize(h->s_d2h); return rc; }
-    aligned = aligned && rows == m;
-    if (total + rows > host_cap) {  // rare: amplification above 2x -- grow the host block, keep the copied prefix
-      RW_CUDA(cudaStreamSynchronize(h->s_d2h));
-      auto o2 = new rwgpu_out();
-      o2->chunk_size = h->chunk_size;
-      const int64_t ncap = (total + rows) * 2;
-      if (!o2->layout(ncap, h->out_types, ~0ull >> 1, true, h->pool)) { delete o2; return fail(RW_ERR_OOM, "pinned output block"); }
-      if (total > 0) {
-        memcpy(o2->ops, o->ops, (size_t)total);
-        for (size_t k = 0; k < h->out_types.size(); k++)
-          if (!type_is_varlen(h->out_types[k])) memcpy(o2->data[k], o->data[k], (size_t)total * type_width(h->out_types[k]));
-      }
-      guard.reset(o2);
-      o = o2;
-      host_cap = ncap;
-    }
-    if (rows > 0) {
-      RW_CUDA(cudaEventRecord(h->ev_main[js], h->stream));
-      RW_CUDA(cudaStreamWaitEvent(h->s_d2h, h->ev_main[js], 0));
-      cudaMemcpyAsync(o->ops + total, h->os().out_ops.as<uint8_t>() + total, (size_t)rows, cudaMemcpyDeviceToHost, h->s_d2h);
-      for (size_t k = 0; k < h->out_types.size(); k++) {
-        if (alias_src[k] >= 0) continue;  // decided after the last sub-batch
-        if (type_is_varlen(h->out_types[k])) continue;  // materialised after the last sub-batch
-        const size_t w = type_width(h->out_types[k]);
-        cudaMemcpyAsync(o->data[k] + (size_t)total * w, h->os().out_col[k].as<uint8_t>() + (size_t)total * w, (size_t)rows * w,
-                        cudaMemcpyDeviceToHost, h->s_d2h);
-      }
-    }
-    total += rows;
-  }
-  rc = join_post_process(h, total, &nullm, h->stream);
-  if (rc != RW_OK) { cudaStreamSynchronize(h->s_d2h); return rc; }
-  if (!h->var_in[side].empty()) {
-    rc = var_check_err(h, h->stream);
-    if (rc != RW_OK) { cudaStreamSynchronize(h->s_d2h); return rc; }
-  }
-  for (int k : h->var_out) {  // handles -> offsets + bytes, then to the host
-    rwgpu_join::VarOut& vo = h->vout[h->cur][k];
-    rc = var_materialize(h, vo, h->os().out_col[k].as<uint64_t>(), (nullm >> 63) ? h->os().out_vis.as<uint8_t>() : nullptr,
-                         ((nullm >> k) & 1) ? h->os().out_valid[k].as<uint8_t>() : nullptr, total, h->stream);
-    if (rc != RW_OK) { cudaStreamSynchronize(h->s_d2h); return rc; }
-    uint8_t* hb = o->var_bytes((size_t)k, vo.total);
-    if (!hb) { cudaStreamSynchronize(h->s_d2h); return fail(RW_ERR_OOM, "pinned varlen output"); }
-    RW_CUDA(cudaMemcpyAsync(o->offsets[k], vo.offs.p, (size_t)(total + 1) * 4, cudaMemcpyDeviceToHost, h->stream));
-    if (vo.total) RW_CUDA(cudaMemcpyAsync(hb, vo.bytes.p, vo.total, cudaMemcpyDeviceToHost, h->stream));
-  }
-  for (size_t k = 0; k < h->out_types.size(); k++) {
-    if (alias_src[k] < 0) continue;
-    if (aligned && total == n) {
-      o->data[k] = (uint8_t*)const_cast<void*>(c->columns[alias_src[k]].data);  // zero-copy: the caller's input column
-    } else if (total > 0) {  // extra matches or an empty sub-batch broke the row alignment: ordinary copy
-      // (every sub-batch's kernels have completed: join_push_dev synchronises on its status read-back)
-      cudaMemcpyAsync(o->data[k], h->os().out_col[k].p, (size_t)total * type_width(h->out_types[k]), cudaMemcpyDeviceToHost, h->s_d2h);
-    }
-  }
-  // NULL / visibility bytes only for the columns that need them (known once all sub-batches ran)
-  if (total > 0) {
-    if (nullm >> 63) cudaMemcpyAsync(o->vis_bytes, h->os().out_vis.p, (size_t)total, cudaMemcpyDeviceToHost, h->s_d2h);
-    for (size_t k = 0; k < h->out_types.size(); k++)
-      if ((nullm >> k) & 1) cudaMemcpyAsync(o->valid_bytes[k], h->os().out_valid[k].p, (size_t)total, cudaMemcpyDeviceToHost, h->s_d2h);
-  }
-  const double t3 = now();
-  RW_CUDA(cudaStreamSynchronize(h->stream));
-  RW_CUDA(cudaStreamSynchronize(h->s_d2h));
-  RW_CUDA(cudaStreamSynchronize(h->s_h2d));
-  const double t4 = now();
-  o->n_rows = total;
-  if (!(nullm >> 63)) o->vis_bytes = nullptr;
-  for (size_t k = 0; k < h->out_types.size(); k++)
-    if (!((nullm >> k) & 1)) o->valid_bytes[k] = nullptr;
-  o->finalize();
-  if (trace)
-    fprintf(stderr, "[rwgpu_join_push] n=%lld out=%lld J=%d  h2d-enqueue %.3f  layout %.3f  sub-batches %.3f  drain %.3f  finalize %.3f  total %.3f ms\n",
-            (long long)n, (long long)total, n_sub, t1 - t0, t2 - t1, t3 - t2, t4 - t3, now() - t4, now() - t0);
-  *out = guard.release();
-  return RW_OK;
-}
+// ---- HOST chunks.  rwgpu_join_push handles one chunk per call and returns when its output sits in host memory: large
+// chunks are cut into sub-batches (multiples of 64 rows, so bitmap words split cleanly) that flow through three streams,
+// H2D of sub-batch j+1 overlapping the kernels of j and the D2H of j-1.  Sub-batches are ordinary consecutive pushes, so
+// the operator semantics are unchanged; their outputs land back to back in one device buffer and one pinned host block.
+// rwgpu_join_push_async only ENQUEUES: input H2D on the copy-in stream, the push on the main stream, and -- the common
+// case being one output row per input row -- the D2H of the positional rows on the set's copy-out stream.  While the
+// caller launches chunk s+1 (its H2D uses the other PCIe direction), chunk s's output streams back; collect waits,
+// copies what the status block says is still missing (extra matches, NULL / visibility bytes) and cuts the chunk views.
 
-// ---- launch / collect split for HOST chunks.  rwgpu_join_push handles one chunk per call and returns when its output
-// sits in host memory: H2D, kernels and D2H of ONE call overlap (sub-batches), consecutive calls do not.  Here the call
-// only ENQUEUES: input H2D on the copy-in stream, the push on the main stream, and -- the common case being one output
-// row per input row -- the D2H of the positional rows on the copy-out stream.  While the caller launches chunk s+1
-// (its H2D uses the other PCIe direction), chunk s's output streams back; collect waits, copies what the status block
-// says is still missing (extra matches, NULL / visibility bytes) and cuts the chunk views.
-int32_t rwgpu_join_push_async(rwgpu_join* h, int32_t side, const rw_chunk* c) {
+static int host_push_check(const rwgpu_join* h, int32_t side, const rw_chunk* c) {
   if (!h || !c) return fail(RW_ERR_INVALID, "null");
   if (side != 0 && side != 1) return fail(RW_ERR_INVALID, "side");
   if (c->n_cols != h->side[side].n_cols) return fail(RW_ERR_INVALID, "chunk schema mismatch");
   for (int k = 0; k < c->n_cols; k++)
     if (c->columns[k].type != h->side[side].types[k]) return fail(RW_ERR_INVALID, "chunk column type mismatch");
+  return RW_OK;
+}
+
+static int host_streams(rwgpu_join* h) {
+  if (h->s_h2d) return RW_OK;
+  RW_CUDA(cudaStreamCreateWithFlags(&h->s_h2d, cudaStreamNonBlocking));
+  RW_CUDA(cudaStreamCreateWithFlags(&h->s_d2h, cudaStreamNonBlocking));
+  for (int i = 0; i < 8; i++) {
+    RW_CUDA(cudaEventCreateWithFlags(&h->ev_h2d[i], cudaEventDisableTiming));
+    RW_CUDA(cudaEventCreateWithFlags(&h->ev_main[i], cudaEventDisableTiming));
+  }
+  for (int i = 0; i < 2; i++) {
+    RW_CUDA(cudaEventCreateWithFlags(&h->ev_up2[i], cudaEventDisableTiming));
+    RW_CUDA(cudaStreamCreateWithFlags(&h->s_out[i], cudaStreamNonBlocking));
+  }
+  return RW_OK;
+}
+
+// A host chunk laid out in an output set's staging (up2 / up2_host), regions sized for the whole chunk: ops, visibility
+// words, then per column its data (varlen: the 8-byte handles) and validity words, plus offsets and bytes for varlen.
+struct HostStage {
+  const rw_chunk* c;
+  uint8_t *dp, *hp;
+  size_t o_ops, o_vis, o_data[RW_MAX_COLS], o_valid[RW_MAX_COLS], o_voff[RW_MAX_COLS], o_vbytes[RW_MAX_COLS];
+  bool pin_ops, pin_col[RW_MAX_COLS];
+};
+
+static int host_stage(rwgpu_join* h, int side, const rw_chunk* c, int set, HostStage* s) {
+  const int64_t n = c->n_rows;
+  const size_t nw = (size_t)((n + 63) / 64) * 8;
+  size_t off = 0;
+  auto region = [&](size_t bytes) { size_t o = align_up_j(off, 256); off = o + bytes; return o; };
+  s->c = c;
+  s->o_ops = region((size_t)n);
+  s->o_vis = region(nw);
+  uint64_t var_bytes_in = 0;  // bytes of the chunk's varlen columns (interned into the side's heap)
+  for (int k = 0; k < c->n_cols; k++) {
+    s->o_data[k] = region((size_t)n * type_width(c->columns[k].type));
+    s->o_valid[k] = region(nw);
+    s->o_voff[k] = s->o_vbytes[k] = 0;
+    if (type_is_varlen(c->columns[k].type)) {
+      if (n && !c->columns[k].offsets) return fail(RW_ERR_INVALID, "varlen column without offsets");
+      const size_t vb = n ? (size_t)(c->columns[k].offsets[n] - c->columns[k].offsets[0]) : 0;
+      s->o_voff[k] = region((size_t)(n + 1) * 4);
+      s->o_vbytes[k] = region(vb + 16);
+      var_bytes_in += vb + 8ull * (uint64_t)n;
+    }
+  }
+  if (var_bytes_in) {
+    int rc = var_ensure_heap(h, side, var_bytes_in);
+    if (rc != RW_OK) return rc;
+    h->var_upper[side] += var_bytes_in;
+  }
+  if (off + 256 > h->up2[set].bytes || off + 256 > h->up2_host[set].bytes) {
+    RW_CUDA(cudaDeviceSynchronize());  // (growth only) an outstanding push may still read the old staging
+    RW_CUDA(h->up2[set].reserve(off + off / 4 + 256));
+    RW_CUDA(h->up2_host[set].reserve(off + off / 4 + 256));
+  }
+  s->dp = h->up2[set].as<uint8_t>();
+  s->hp = h->up2_host[set].as<uint8_t>();
+  auto is_pinned = [&](const void* p) {
+    if (!n) return false;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return a.type == cudaMemoryTypeHost;
+  };
+  s->pin_ops = is_pinned(c->ops);
+  for (int k = 0; k < c->n_cols; k++) s->pin_col[k] = is_pinned(c->columns[k].data);
+  return RW_OK;
+}
+
+// H2D of rows [lo, lo + m) on s_h2d.  A caller buffer that is already pinned is copied straight from user memory;
+// pageable small pieces go through the pinned staging (one memcpy), pageable large ones directly.
+static void host_stage_upload(rwgpu_join* h, const HostStage& s, int64_t lo, int64_t m) {
+  const rw_chunk* c = s.c;
+  auto h2d = [&](size_t dst_off, const void* src, size_t bytes, bool pinned) {
+    if (!bytes) return;
+    if (pinned || bytes >= (1u << 20)) cudaMemcpyAsync(s.dp + dst_off, src, bytes, cudaMemcpyHostToDevice, h->s_h2d);
+    else { memcpy(s.hp + dst_off, src, bytes); cudaMemcpyAsync(s.dp + dst_off, s.hp + dst_off, bytes, cudaMemcpyHostToDevice, h->s_h2d); }
+  };
+  const size_t wlo = (size_t)(lo / 64) * 8, wn = (size_t)((m + 63) / 64) * 8;
+  h2d(s.o_ops + (size_t)lo, c->ops + lo, (size_t)m, s.pin_ops);
+  if (c->visibility) h2d(s.o_vis + wlo, (const uint8_t*)c->visibility + wlo, wn, false);
+  for (int k = 0; k < c->n_cols; k++) {
+    const int w = type_width(c->columns[k].type);
+    if (type_is_varlen(c->columns[k].type)) {  // offsets lo .. lo+m and the bytes they span
+      const uint32_t* of = c->columns[k].offsets;
+      h2d(s.o_voff[k] + (size_t)lo * 4, of + lo, (size_t)(m + 1) * 4, false);
+      h2d(s.o_vbytes[k] + (size_t)(of[lo] - of[0]), (const uint8_t*)c->columns[k].data + of[lo], (size_t)(of[lo + m] - of[lo]), s.pin_col[k]);
+    } else {
+      h2d(s.o_data[k] + (size_t)lo * w, (const uint8_t*)c->columns[k].data + (size_t)lo * w, (size_t)m * w, s.pin_col[k]);
+    }
+    if (c->columns[k].validity) h2d(s.o_valid[k] + wlo, (const uint8_t*)c->columns[k].validity + wlo, wn, false);
+  }
+}
+
+// the staged rows [lo, lo + m) as a device chunk (lo a multiple of 64)
+static DevChunk host_stage_chunk(const HostStage& s, int64_t lo, int64_t m) {
+  const rw_chunk* c = s.c;
+  DevChunk ch;
+  memset(&ch, 0, sizeof(ch));
+  ch.n = m;
+  ch.n_cols = c->n_cols;
+  ch.ops = s.dp + s.o_ops + lo;
+  ch.vis_bits = c->visibility ? (const uint64_t*)(s.dp + s.o_vis + (size_t)(lo / 64) * 8) : nullptr;
+  for (int k = 0; k < c->n_cols; k++) {
+    const int w = type_width(c->columns[k].type);
+    ch.cols[k].type = c->columns[k].type;
+    ch.cols[k].width = w;
+    ch.cols[k].data = s.dp + s.o_data[k] + (size_t)lo * w;
+    ch.cols[k].valid_bits = c->columns[k].validity ? (const uint64_t*)(s.dp + s.o_valid[k] + (size_t)(lo / 64) * 8) : nullptr;
+  }
+  return ch;
+}
+
+// Positional inner-join output (row r of the output = input row r): the update side's output columns are byte-for-byte
+// the caller's input columns, which already sit in host memory -- they are not copied back over PCIe; the output chunk
+// views alias the input buffers instead (contract in rwgpu.h).  Output column -> input column, -1 = copied back.
+static std::vector<int> host_alias_src(const rwgpu_join* h, int side, const rw_chunk* c) {
+  std::vector<int> src(h->out_types.size(), -1);
+  bool ok = h->w8_ok[side] && !c->visibility && c->n_rows > 0;
+  for (int k = 0; k < c->n_cols && ok; k++) ok = c->columns[k].validity == nullptr;
+  if (ok)
+    for (int k = 0; k < c->n_cols; k++)
+      if (h->w8[side].u_out[k] >= 0 && !type_is_varlen(c->columns[k].type)) src[(size_t)h->w8[side].u_out[k]] = k;
+  return src;
+}
+
+// A pinned output block for `rows` rows, with room for twice as many (at least 1024; *cap), holding the first `keep`
+// rows of ops and fixed-width columns of `old`.  nullptr on OOM.
+static rwgpu_out* host_out_block(rwgpu_join* h, int64_t rows, int64_t* cap, const rwgpu_out* old = nullptr, int64_t keep = 0) {
+  std::unique_ptr<rwgpu_out> o(new rwgpu_out());
+  o->chunk_size = h->chunk_size;
+  *cap = std::max<int64_t>(2 * rows, 1024);
+  if (!o->layout(*cap, h->out_types, ~0ull >> 1, true, h->pool)) return nullptr;
+  if (keep > 0) {
+    memcpy(o->ops, old->ops, (size_t)keep);
+    for (size_t k = 0; k < h->out_types.size(); k++)
+      if (!type_is_varlen(h->out_types[k])) memcpy(o->data[k], old->data[k], (size_t)keep * type_width(h->out_types[k]));
+  }
+  return o.release();
+}
+
+// D2H on `sd` of output rows [lo, hi): ops and the fixed-width columns that are not aliased
+static void host_out_copy(rwgpu_join* h, rwgpu_out* o, const std::vector<int>& alias_src, int64_t lo, int64_t hi, cudaStream_t sd) {
+  cudaMemcpyAsync(o->ops + lo, h->os().out_ops.as<uint8_t>() + lo, (size_t)(hi - lo), cudaMemcpyDeviceToHost, sd);
+  for (size_t k = 0; k < h->out_types.size(); k++) {
+    if (alias_src[k] >= 0 || type_is_varlen(h->out_types[k])) continue;  // (varlen columns are materialised at the end)
+    const size_t w = type_width(h->out_types[k]);
+    cudaMemcpyAsync(o->data[k] + (size_t)lo * w, h->os().out_col[k].as<uint8_t>() + (size_t)lo * w, (size_t)(hi - lo) * w, cudaMemcpyDeviceToHost, sd);
+  }
+}
+
+// The end of a host-chunk push: on `sd`, whatever `o` still lacks of the current output set's first `total` rows --
+// rows [from, total) of each copied fixed-width column, an aliased column whole unless `aligned` (output row r is input
+// row r) lets it point at the caller's column, the visibility / validity bytes `nullm` flags -- then the block is cut,
+// once `sd` and `main_st` (if given: copies of varlen columns may still run there) are drained.
+static int host_out_finish(rwgpu_join* h, rwgpu_out* o, const rw_column* in_cols, const std::vector<int>& alias_src, bool aligned, int64_t from,
+                           int64_t total, unsigned long long nullm, cudaStream_t sd, cudaStream_t main_st = nullptr) {
+  for (size_t k = 0; k < h->out_types.size(); k++) {
+    if (type_is_varlen(h->out_types[k])) continue;  // materialised by the caller
+    const bool alias = alias_src[k] >= 0;
+    if (alias && aligned) {
+      o->data[k] = (uint8_t*)const_cast<void*>(in_cols[alias_src[k]].data);  // zero-copy
+      continue;
+    }
+    const int64_t lo = alias ? 0 : from;
+    const size_t w = type_width(h->out_types[k]);
+    if (total > lo)
+      cudaMemcpyAsync(o->data[k] + (size_t)lo * w, h->os().out_col[k].as<uint8_t>() + (size_t)lo * w, (size_t)(total - lo) * w, cudaMemcpyDeviceToHost, sd);
+  }
+  if (total > 0) {
+    if (nullm >> 63) cudaMemcpyAsync(o->vis_bytes, h->os().out_vis.p, (size_t)total, cudaMemcpyDeviceToHost, sd);
+    for (size_t k = 0; k < h->out_types.size(); k++)
+      if ((nullm >> k) & 1) cudaMemcpyAsync(o->valid_bytes[k], h->os().out_valid[k].p, (size_t)total, cudaMemcpyDeviceToHost, sd);
+  }
+  if (main_st) RW_CUDA(cudaStreamSynchronize(main_st));
+  RW_CUDA(cudaStreamSynchronize(sd));
+  o->n_rows = total;
+  if (!(nullm >> 63)) o->vis_bytes = nullptr;
+  for (size_t k = 0; k < h->out_types.size(); k++)
+    if (!((nullm >> k) & 1)) o->valid_bytes[k] = nullptr;
+  o->finalize();
+  return RW_OK;
+}
+
+int32_t rwgpu_join_push(rwgpu_join* h, int32_t side, const rw_chunk* c, rwgpu_out** out) {
+  if (!out) return fail(RW_ERR_INVALID, "null");
+  int rc = host_push_check(h, side, c);
+  if (rc != RW_OK) return rc;
+  if (h->n_pending) return fail(RW_ERR_INVALID, "collect the outstanding asynchronous pushes first");
+  const int64_t n = c->n_rows;
+  rc = host_streams(h);
+  if (rc != RW_OK) return rc;
+  // each sub-batch costs one status read-back: keep them >= 32K rows
+  const int J = n >= (1 << 19) ? 8 : (n >= (1 << 17) ? 4 : (n >= (1 << 16) ? 2 : 1));
+  int64_t sub = (n + J - 1) / J;
+  sub = (sub + 63) / 64 * 64;
+  HostStage s;
+  rc = host_stage(h, side, c, h->cur, &s);
+  if (rc != RW_OK) return rc;
+  RW_CUDA(cudaStreamSynchronize(h->s_d2h));  // previous call's copies are long done; cheap guard for buffer reuse
+  // enqueue every sub-batch's H2D up front
+  int n_sub = 0;
+  for (int64_t lo = 0; lo < n; lo += sub, n_sub++) {
+    host_stage_upload(h, s, lo, std::min<int64_t>(sub, n - lo));
+    RW_CUDA(cudaEventRecord(h->ev_h2d[n_sub], h->s_h2d));
+  }
+  RW_CUDA(cudaGetLastError());
+  rc = join_begin_call(h, h->stream);
+  if (rc != RW_OK) return rc;
+  int64_t host_cap;
+  std::unique_ptr<rwgpu_out> o(host_out_block(h, n, &host_cap));
+  if (!o) return fail(RW_ERR_OOM, "pinned output block");
+  const std::vector<int> alias_src = host_alias_src(h, side, c);
+  bool aligned = true;  // every sub-batch produced exactly its positional rows (no extras, no empty result)
+  int64_t total = 0;
+  unsigned long long nullm = 0;
+  auto bail = [&](int rc) { cudaStreamSynchronize(h->s_d2h); return rc; };  // copies into `o` may be in flight
+  int js = 0;
+  for (int64_t lo = 0; lo < n; lo += sub, js++) {
+    const int64_t m = std::min<int64_t>(sub, n - lo);
+    const DevChunk ch = host_stage_chunk(s, lo, m);
+    RW_CUDA(cudaStreamWaitEvent(h->stream, h->ev_h2d[js], 0));
+    for (int k : h->var_in[side]) {  // bytes -> the side's heap, the column becomes a column of handles
+      rc = var_intern(h, side, s.dp + s.o_vbytes[k] - c->columns[k].offsets[0], (const uint32_t*)(s.dp + s.o_voff[k]) + lo, ch.ops, ch.vis_bits,
+                      ch.cols[k].valid_bits, m, (uint64_t*)(s.dp + s.o_data[k]) + lo, h->stream);
+      if (rc != RW_OK) return bail(rc);
+    }
+    int64_t rows = 0;
+    rc = join_push_dev(h, side, ch, h->stream, total, &rows, &nullm);
+    if (rc != RW_OK) return bail(rc);
+    aligned = aligned && rows == m;
+    if (total + rows > host_cap) {  // rare: amplification above 2x -- grow the host block, keep the copied prefix
+      RW_CUDA(cudaStreamSynchronize(h->s_d2h));
+      rwgpu_out* o2 = host_out_block(h, total + rows, &host_cap, o.get(), total);
+      if (!o2) return fail(RW_ERR_OOM, "pinned output block");
+      o.reset(o2);
+    }
+    if (rows > 0) {
+      RW_CUDA(cudaEventRecord(h->ev_main[js], h->stream));
+      RW_CUDA(cudaStreamWaitEvent(h->s_d2h, h->ev_main[js], 0));
+      host_out_copy(h, o.get(), alias_src, total, total + rows, h->s_d2h);  // (aliased columns: decided after the last sub-batch)
+    }
+    total += rows;
+  }
+  rc = join_post_process(h, total, &nullm, h->stream);
+  if (rc != RW_OK) return bail(rc);
+  if (!h->var_in[side].empty()) {
+    rc = var_check_err(h, h->stream);
+    if (rc != RW_OK) return bail(rc);
+  }
+  for (int k : h->var_out) {  // handles -> offsets + bytes, then to the host
+    rwgpu_join::VarOut& vo = h->vout[h->cur][k];
+    rc = var_materialize(h, vo, h->os().out_col[k].as<uint64_t>(), (nullm >> 63) ? h->os().out_vis.as<uint8_t>() : nullptr,
+                         ((nullm >> k) & 1) ? h->os().out_valid[k].as<uint8_t>() : nullptr, total, h->stream);
+    if (rc != RW_OK) return bail(rc);
+    uint8_t* hb = o->var_bytes((size_t)k, vo.total);
+    if (!hb) return bail(fail(RW_ERR_OOM, "pinned varlen output"));
+    RW_CUDA(cudaMemcpyAsync(o->offsets[k], vo.offs.p, (size_t)(total + 1) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (vo.total) RW_CUDA(cudaMemcpyAsync(hb, vo.bytes.p, vo.total, cudaMemcpyDeviceToHost, h->stream));
+  }
+  // (every sub-batch's kernels have completed: join_push_dev synchronises on its status read-back)
+  rc = host_out_finish(h, o.get(), c->columns, alias_src, aligned && total == n, total, total, nullm, h->s_d2h, h->stream);
+  if (rc != RW_OK) return rc;
+  RW_CUDA(cudaStreamSynchronize(h->s_h2d));
+  *out = o.release();
+  return RW_OK;
+}
+
+int32_t rwgpu_join_push_async(rwgpu_join* h, int32_t side, const rw_chunk* c) {
+  int rc = host_push_check(h, side, c);
+  if (rc != RW_OK) return rc;
   if (h->n_pending >= 2) return fail(RW_ERR_INVALID, "two pushes are already outstanding: collect one first");
   if (h->n_pending && h->pending[0].S != side)
     return fail(RW_ERR_INVALID, "pushes of different sides cannot be outstanding together: collect first");
@@ -3057,118 +3085,48 @@ int32_t rwgpu_join_push_async(rwgpu_join* h, int32_t side, const rw_chunk* c) {
   const int set = h->n_pending ? 1 - h->pending[h->n_pending - 1].set : h->cur;
   rwgpu_join::HostPending& hp = h->hpend[set];
   if (hp.active) return fail(RW_ERR_INVALID, "output set still holds an uncollected host push");
-  hp = rwgpu_join::HostPending();
-  hp.active = true;
-  hp.n = n;
-  hp.in = *c;
-  hp.in_cols.assign(c->columns, c->columns + c->n_cols);
-  hp.in.columns = hp.in_cols.data();
   JoinPending pd;
   pd.S = side;
   pd.set = set;
   pd.st = h->stream;
-  bool simple = h->uni && n > 0 && n < (1ll << 31) && h->var_in[side].empty() && h->var_out.empty();
-  if (!simple) {
+  hp = rwgpu_join::HostPending();
+  hp.in_cols.assign(c->columns, c->columns + c->n_cols);
+  hp.n = n;
+  std::unique_ptr<rwgpu_out> o;
+  if (!(h->uni && n > 0 && n < (1ll << 31) && h->var_in[side].empty() && h->var_out.empty())) {
     // other plan shapes / varlen payload / empty chunks: run the synchronous call now, hand the result over at collect
     if (h->n_pending) return fail(RW_ERR_INVALID, "this join shape runs its pushes synchronously: collect the outstanding push first");
-    hp.active = false;
-    rwgpu_out* o = nullptr;
-    int rc = rwgpu_join_push(h, side, c, &o);
+    rwgpu_out* so = nullptr;
+    rc = rwgpu_join_push(h, side, c, &so);
     if (rc != RW_OK) return rc;
-    hp.active = true;
-    hp.sync_done = true;
-    hp.out = o;
+    o.reset(so);
     pd.sync_done = true;  // (nothing is outstanding: `set` is the current set)
-    h->pending[h->n_pending++] = pd;
-    return RW_OK;
+  } else {
+    rc = host_streams(h);
+    if (rc != RW_OK) return rc;
+    HostStage s;
+    rc = host_stage(h, side, c, set, &s);
+    if (rc != RW_OK) return rc;
+    // (the copy-in stream is ordered behind the kernels that read this staging two pushes ago: that push was collected)
+    host_stage_upload(h, s, 0, n);
+    RW_CUDA(cudaEventRecord(h->ev_up2[set], h->s_h2d));
+    RW_CUDA(cudaGetLastError());
+    h->cur = set;
+    rc = join_begin_call(h, h->stream);
+    if (rc != RW_OK) return rc;
+    RW_CUDA(cudaStreamWaitEvent(h->stream, h->ev_up2[set], 0));
+    rc = uni_enqueue(h, side, host_stage_chunk(s, 0, n), h->stream, 0, false, &pd);
+    if (rc != RW_OK) return rc;
+    // the output block and the copy-out of the positional rows
+    o.reset(host_out_block(h, n, &hp.host_cap));
+    if (!o) return fail(RW_ERR_OOM, "pinned output block");
+    hp.alias_src = host_alias_src(h, side, c);
+    RW_CUDA(cudaStreamWaitEvent(h->s_out[set], h->pend_ev[set], 0));
+    host_out_copy(h, o.get(), hp.alias_src, 0, n, h->s_out[set]);
+    RW_CUDA(cudaGetLastError());
   }
-  if (!h->s_h2d) {
-    RW_CUDA(cudaStreamCreateWithFlags(&h->s_h2d, cudaStreamNonBlocking));
-    RW_CUDA(cudaStreamCreateWithFlags(&h->s_d2h, cudaStreamNonBlocking));
-    for (int i = 0; i < 8; i++) {
-      RW_CUDA(cudaEventCreateWithFlags(&h->ev_h2d[i], cudaEventDisableTiming));
-      RW_CUDA(cudaEventCreateWithFlags(&h->ev_main[i], cudaEventDisableTiming));
-    }
-  }
-  if (!h->ev_up2[set]) RW_CUDA(cudaEventCreateWithFlags(&h->ev_up2[set], cudaEventDisableTiming));
-  if (!h->s_out[set]) RW_CUDA(cudaStreamCreateWithFlags(&h->s_out[set], cudaStreamNonBlocking));
-  cudaStream_t sd = h->s_out[set];
-  // ---- input: device staging of this set
-  const size_t nw = (size_t)((n + 63) / 64) * 8;
-  size_t off = 0;
-  auto region = [&](size_t bytes) { size_t o = align_up_j(off, 256); off = o + bytes; return o; };
-  const size_t o_ops = region((size_t)n), o_vis = region(nw);
-  size_t o_data[RW_MAX_COLS], o_valid[RW_MAX_COLS];
-  for (int k = 0; k < c->n_cols; k++) {
-    o_data[k] = region((size_t)n * type_width(c->columns[k].type));
-    o_valid[k] = region(nw);
-  }
-  if (off + 256 > h->up2[set].bytes) {
-    RW_CUDA(cudaDeviceSynchronize());  // (growth only)
-    RW_CUDA(h->up2[set].reserve(off + off / 4 + 256));
-    RW_CUDA(h->up2_host[set].reserve(off + off / 4 + 256));
-  }
-  uint8_t* hs = h->up2_host[set].as<uint8_t>();
-  uint8_t* dp = h->up2[set].as<uint8_t>();
-  auto is_pinned = [](const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeHost;
-  };
-  // (the copy-in stream is ordered behind the kernels that read this staging two pushes ago: that push was collected)
-  auto h2d = [&](size_t dst_off, const void* src, size_t bytes, bool pinned) {
-    if (!bytes) return;
-    if (pinned || bytes >= (1u << 20)) cudaMemcpyAsync(dp + dst_off, src, bytes, cudaMemcpyHostToDevice, h->s_h2d);
-    else { memcpy(hs + dst_off, src, bytes); cudaMemcpyAsync(dp + dst_off, hs + dst_off, bytes, cudaMemcpyHostToDevice, h->s_h2d); }
-  };
-  h2d(o_ops, c->ops, (size_t)n, is_pinned(c->ops));
-  if (c->visibility) h2d(o_vis, c->visibility, nw, false);
-  for (int k = 0; k < c->n_cols; k++) {
-    h2d(o_data[k], c->columns[k].data, (size_t)n * type_width(c->columns[k].type), is_pinned(c->columns[k].data));
-    if (c->columns[k].validity) h2d(o_valid[k], c->columns[k].validity, nw, false);
-  }
-  RW_CUDA(cudaEventRecord(h->ev_up2[set], h->s_h2d));
-  RW_CUDA(cudaGetLastError());
-  DevChunk ch;
-  memset(&ch, 0, sizeof(ch));
-  ch.n = n;
-  ch.n_cols = c->n_cols;
-  ch.ops = dp + o_ops;
-  ch.vis_bits = c->visibility ? (const uint64_t*)(dp + o_vis) : nullptr;
-  for (int k = 0; k < c->n_cols; k++) {
-    ch.cols[k].type = c->columns[k].type;
-    ch.cols[k].width = type_width(c->columns[k].type);
-    ch.cols[k].data = dp + o_data[k];
-    ch.cols[k].valid_bits = c->columns[k].validity ? (const uint64_t*)(dp + o_valid[k]) : nullptr;
-  }
-  // ---- the push
-  h->cur = set;
-  int rc = join_begin_call(h, h->stream);
-  if (rc != RW_OK) { hp.active = false; return rc; }
-  RW_CUDA(cudaStreamWaitEvent(h->stream, h->ev_up2[set], 0));
-  rc = uni_enqueue(h, side, ch, h->stream, 0, false, &pd);
-  if (rc != RW_OK) { hp.active = false; return rc; }
-  // ---- output block + the copy-out of the positional rows
-  auto o = new rwgpu_out();
-  o->chunk_size = h->chunk_size;
-  hp.host_cap = std::max<int64_t>(2 * n, 1024);
-  if (!o->layout(hp.host_cap, h->out_types, ~0ull >> 1, true, h->pool)) { delete o; hp.active = false; return fail(RW_ERR_OOM, "pinned output block"); }
-  hp.out = o;
-  static const bool no_alias = getenv("RWGPU_NO_ALIAS") != nullptr;
-  hp.alias_ok = !no_alias && h->w8_ok[side] && !c->visibility;
-  for (int k = 0; k < c->n_cols && hp.alias_ok; k++) hp.alias_ok = c->columns[k].validity == nullptr;
-  hp.alias_src.assign(h->out_types.size(), -1);
-  if (hp.alias_ok)
-    for (int k = 0; k < c->n_cols; k++)
-      if (h->w8[side].u_out[k] >= 0) hp.alias_src[(size_t)h->w8[side].u_out[k]] = k;
-  RW_CUDA(cudaStreamWaitEvent(sd, h->pend_ev[set], 0));
-  cudaMemcpyAsync(o->ops, h->os().out_ops.p, (size_t)n, cudaMemcpyDeviceToHost, sd);
-  for (size_t k = 0; k < h->out_types.size(); k++) {
-    if (hp.alias_src[k] >= 0) continue;
-    const size_t w = type_width(h->out_types[k]);
-    cudaMemcpyAsync(o->data[k], h->os().out_col[k].p, (size_t)n * w, cudaMemcpyDeviceToHost, sd);
-  }
-  RW_CUDA(cudaGetLastError());
+  hp.active = true;
+  hp.out = o.release();
   h->pending[h->n_pending++] = pd;
   return RW_OK;
 }
@@ -3182,14 +3140,13 @@ int32_t rwgpu_join_collect_out(rwgpu_join* h, rwgpu_out** out) {
   h->pending[0] = h->pending[1];
   h->n_pending--;
   hp.active = false;
-  if (hp.sync_done) {
+  if (pd.sync_done) {
     *out = hp.out;
     hp.out = nullptr;
     return RW_OK;
   }
-  std::unique_ptr<rwgpu_out> guard(hp.out);
+  std::unique_ptr<rwgpu_out> o(hp.out);
   hp.out = nullptr;
-  rwgpu_out* o = guard.get();
   cudaStream_t sd = h->s_out[pd.set];
   h->cur = pd.set;
   h->call_null_mask = 0;
@@ -3211,41 +3168,19 @@ int32_t rwgpu_join_collect_out(rwgpu_join* h, rwgpu_out** out) {
   bool pre_ok = h->os().out_ops.as<uint8_t>() == ops_before && total >= n;
   if (total > hp.host_cap) {  // rare: amplification above 2x -- a larger host block, everything is copied again
     RW_CUDA(cudaStreamSynchronize(sd));
-    auto o2 = new rwgpu_out();
-    o2->chunk_size = h->chunk_size;
-    if (!o2->layout(total + total / 4, h->out_types, ~0ull >> 1, true, h->pool)) { delete o2; return bail(fail(RW_ERR_OOM, "pinned output block")); }
-    guard.reset(o2);
-    o = o2;
+    o.reset(host_out_block(h, total, &hp.host_cap));
+    if (!o) return bail(fail(RW_ERR_OOM, "pinned output block"));
     pre_ok = false;
   }
-  const bool aligned = total == n;  // exactly the positional rows: the update side's columns ARE the caller's input columns
-  if (total > 0) {
-    const int64_t from = pre_ok ? n : 0;  // rows [0, n) of the non-aliased columns are already on their way
-    const int64_t ops_from = h->call_had_deletes ? 0 : from;  // (the no-op elimination pass may have rewritten ops)
-    if (total > ops_from)
-      cudaMemcpyAsync(o->ops + ops_from, h->os().out_ops.as<uint8_t>() + ops_from, (size_t)(total - ops_from), cudaMemcpyDeviceToHost, sd);
-    for (size_t k = 0; k < h->out_types.size(); k++) {
-      const size_t w = type_width(h->out_types[k]);
-      if (hp.alias_src[k] >= 0) {
-        if (aligned) o->data[k] = (uint8_t*)const_cast<void*>(hp.in_cols[(size_t)hp.alias_src[k]].data);  // zero-copy
-        else cudaMemcpyAsync(o->data[k], h->os().out_col[k].p, (size_t)total * w, cudaMemcpyDeviceToHost, sd);
-      } else if (total > from) {
-        cudaMemcpyAsync(o->data[k] + (size_t)from * w, h->os().out_col[k].as<uint8_t>() + (size_t)from * w, (size_t)(total - from) * w,
-                        cudaMemcpyDeviceToHost, sd);
-      }
-    }
-    if (nullm >> 63) cudaMemcpyAsync(o->vis_bytes, h->os().out_vis.p, (size_t)total, cudaMemcpyDeviceToHost, sd);
-    for (size_t k = 0; k < h->out_types.size(); k++)
-      if ((nullm >> k) & 1) cudaMemcpyAsync(o->valid_bytes[k], h->os().out_valid[k].p, (size_t)total, cudaMemcpyDeviceToHost, sd);
-  }
-  RW_CUDA(cudaStreamSynchronize(sd));
-  o->n_rows = total;
-  if (!(nullm >> 63)) o->vis_bytes = nullptr;
-  for (size_t k = 0; k < h->out_types.size(); k++)
-    if (!((nullm >> k) & 1)) o->valid_bytes[k] = nullptr;
-  o->finalize();
+  const int64_t from = pre_ok ? n : 0;  // rows [0, n) of the non-aliased columns are already on their way
+  const int64_t ops_from = h->call_had_deletes ? 0 : from;  // (the no-op elimination pass may have rewritten ops)
+  if (total > ops_from)
+    cudaMemcpyAsync(o->ops + ops_from, h->os().out_ops.as<uint8_t>() + ops_from, (size_t)(total - ops_from), cudaMemcpyDeviceToHost, sd);
+  // exactly the positional rows: the update side's columns ARE the caller's input columns
+  rc = host_out_finish(h, o.get(), hp.in_cols.data(), hp.alias_src, total == n, from, total, nullm, sd);
+  if (rc != RW_OK) return bail(rc);
   if (h->n_pending) h->cur = h->pending[h->n_pending - 1].set;
-  *out = guard.release();
+  *out = o.release();
   return RW_OK;
 }
 

@@ -10,7 +10,6 @@
 #include <cooperative_groups.h>
 
 #include <algorithm>
-#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -881,23 +880,10 @@ int32_t rwgpu_shuffle_partition_p2p_device(const rw_chunk* c, const int32_t* key
   uint8_t* dest = scratch;
   uint32_t* hist = (uint32_t*)(scratch + dest_bytes);
   int64_t* offsets = (int64_t*)(scratch + dest_bytes + (hist_bytes + 255) / 256 * 256);
-  static const bool trace = getenv("RWGPU_TRACE") != nullptr;  // per-kernel wall clock (adds syncs)
-  auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  double t0 = 0, t1 = 0, t2 = 0, t3 = 0, t4 = 0;
-  if (trace) { cudaStreamSynchronize(st); t0 = now(); }
   part_hist_kernel<<<n_blocks, PART_BLOCK, 0, st>>>(ch, p, vnode_to_dest, n_dest, dest, hist);
-  if (trace) { cudaStreamSynchronize(st); t1 = now(); }
   part_scan_kernel<<<1, PART_SCAN_THREADS, 0, st>>>(hist, n_blocks, n_dest, counts, offsets);
-  if (trace) { cudaStreamSynchronize(st); t2 = now(); }
   part_scatter_p2p_kernel<<<n_blocks, PART_BLOCK, 0, st>>>(ch, dest, hist, n_dest, L, pb, my_rank, overflow);
-  if (trace) { cudaStreamSynchronize(st); t3 = now(); }
   p2p_publish_counts_kernel<<<1, PART_MAX_DEST, 0, st>>>(counts, n_dest, L, pb, my_rank);
-  if (trace) {
-    cudaStreamSynchronize(st);
-    t4 = now();
-    fprintf(stderr, "  [p2p partition n=%lld] hist %.3f  scan %.3f  scatter %.3f  publish %.3f ms\n", (long long)c->n_rows, t1 - t0, t2 - t1,
-            t3 - t2, t4 - t3);
-  }
   RW_CUDA(cudaGetLastError());
   RW_CUDA(cudaFreeAsync(scratch, st));
   return RW_OK;
@@ -916,13 +902,8 @@ int32_t rwgpu_shuffle_exchange_p2p_device(const rw_chunk* c, const int32_t* keys
   PeerBases pf;
   memset(&pf, 0, sizeof(pf));
   for (int d = 0; d < n_dest; d++) pf.base[d] = (uint8_t*)peer_flags[d];
-  static const bool trace = getenv("RWGPU_TRACE") != nullptr;
-  auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  double t0 = 0, t1 = 0;
-  if (trace) { cudaStreamSynchronize(st); t0 = now(); }
   p2p_barrier_kernel<<<1, PART_MAX_DEST, 0, st>>>(pf, n_dest, my_rank, (unsigned long long)epoch);
   RW_CUDA(cudaGetLastError());
-  if (trace) { cudaStreamSynchronize(st); t1 = now(); }
   std::vector<int32_t> types(c->n_cols);
   for (int k = 0; k < c->n_cols; k++) types[k] = c->columns[k].type;
   // the device-side row count lives behind the flags of this rank's block: byte 512 + 8 * (epoch & 1)
@@ -932,10 +913,6 @@ int32_t rwgpu_shuffle_exchange_p2p_device(const rw_chunk* c, const int32_t* keys
   if (rc != RW_OK) return rc;
   p2p_total_to_host_kernel<<<1, 1, 0, st>>>(total_dev, total_host);
   RW_CUDA(cudaGetLastError());
-  if (trace) {
-    cudaStreamSynchronize(st);
-    fprintf(stderr, "  [p2p exchange] barrier (incl. waiting for the peers) %.3f  unpack + count %.3f ms\n", t1 - t0, now() - t1);
-  }
   return RW_OK;
 }
 
