@@ -458,11 +458,17 @@ int32_t rwgpu_filter_device(const rw_chunk* chunk, const rw_filter_term* terms, 
  * Replaces apply_project_exprs                   src/stream/src/executor/project/project_scalar.rs:91-108
  * for INTEGER expressions in postfix form.  An InputRef projection needs no call at all (re-order the column
  * pointers).  Evaluation is non-strict like the reference's (`eval_infallible`): a NULL operand, a numeric overflow
- * (checked_add / checked_sub / checked_mul, also of the narrower result type) or a division by zero makes the ROW's
- * value NULL, never an error.  Ops and visibility of the chunk pass through unchanged.
+ * (checked_add / checked_sub / checked_mul / checked_div / checked_neg of the OPERATION's result type), MIN % -1
+ * (checked_rem) or a division by zero makes the ROW's value NULL, never an error.  Ops and visibility of the chunk
+ * pass through unchanged.
  *   RW_EX_COL    push column `arg` (Int16/32/64, Date, Time, Timestamp(tz), Serial)      RW_EX_CONST  push `value`
  *   RW_EX_ADD / SUB / MUL / DIV / MOD (b = pop, a = pop, push a op b; Rust semantics: truncating /, sign of a for %)
- *   RW_EX_NEG    RW_EX_TUMBLE_START / RW_EX_TUMBLE_END  (a = timestamp in us, b = window in us; tumble.rs:91-112)
+ *   RW_EX_NEG    RW_EX_TUMBLE_START / RW_EX_TUMBLE_END  (a = timestamp in us, or a DATE operand (days), which becomes
+ *                the timestamp of its midnight; b = window in us; tumble.rs:34-112)
+ * Every operator (RW_EX_ADD..RW_EX_NEG) carries its result type in `arg`: an integer-typed RW_T_*, 0 = RW_T_INT64.
+ * The result of the operation must fit that type (Int16 / Int32 / Date: 2 / 4 / 4 bytes, the others 8), else the row is
+ * NULL.  An `arg` that is no RW_T_* is RW_ERR_INVALID.  The device evaluates at most 16 expressions of at most 24
+ * operations and a stack depth of 8 (RW_ERR_UNSUPPORTED beyond).
  * Everything else the expression framework can evaluate stays on the CPU ProjectExecutor.                       */
 #define RW_EX_COL 1
 #define RW_EX_CONST 2
@@ -476,7 +482,7 @@ int32_t rwgpu_filter_device(const rw_chunk* chunk, const rw_filter_term* terms, 
 #define RW_EX_NEG 10
 typedef struct rw_expr_op {
   int32_t op;     /* RW_EX_*                         */
-  int32_t arg;    /* RW_EX_COL: input column          */
+  int32_t arg;    /* RW_EX_COL: input column; operator: result RW_T_* (0 = INT64) */
   int64_t value;  /* RW_EX_CONST                     */
 } rw_expr_op;
 typedef struct rw_project_expr {

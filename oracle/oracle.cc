@@ -1094,9 +1094,11 @@ extern "C" int32_t rwo_agg_eval(const rw_agg_call* call, int32_t arg_type, const
 // ================================================================== Project
 // apply_project_exprs (src/stream/src/executor/project/project_scalar.rs:91-108) for integer expressions in postfix
 // form (include/rwgpu.h RW_EX_*): NonStrictExpression::eval_infallible -- a NULL operand or a failed evaluation
-// (checked_add / checked_sub / checked_mul overflow: src/expr/impl/src/scalar/arithmetic_op.rs general_*; division by
-// zero; a result that does not fit the expression's integer type) makes the row's value NULL.  tumble_start:
-// src/expr/impl/src/scalar/tumble.rs:91-112 (get_window_start_with_offset, zero offset); tumble_end = start + window.
+// (checked_add / checked_sub / checked_mul / checked_neg overflow of the operation's own result type `arg`:
+// src/expr/impl/src/scalar/arithmetic_op.rs general_*; division by zero; MIN % -1 (checked_rem); a result that does not
+// fit the expression's integer type) makes the row's value NULL.  tumble_start: src/expr/impl/src/scalar/tumble.rs:91-112
+// (get_window_start_with_offset, zero offset), over a DATE the timestamp of its midnight (:34-37); tumble_end = start +
+// window.
 extern "C" int32_t rwo_project(const rw_chunk* ch, const rw_project_expr* exprs, int32_t n_exprs, void* const* out_data,
                                uint64_t* const* out_validity, uint32_t* has_null) {
   const int64_t n = ch->n_rows;
@@ -1107,10 +1109,47 @@ extern "C" int32_t rwo_project(const rw_chunk* ch, const rw_project_expr* exprs,
       default: return false;
     }
   };
+  auto type_min = [](int t) -> i128 {
+    const int w = type_width(t);
+    return w == 2 ? (i128)INT16_MIN : w == 4 ? (i128)INT32_MIN : (i128)INT64_MIN;
+  };
   if (n_exprs < 1 || n_exprs > 16) { g_err = "project: 1..16 expressions"; return RW_ERR_UNSUPPORTED; }
+  // validate every program first (also for an empty chunk); op_type[e][k]: result type of an operation, op_date[e][k]:
+  // its first operand is a DATE
+  std::vector<std::vector<int>> op_type(n_exprs), op_date(n_exprs);
   for (int e = 0; e < n_exprs; e++) {
     const rw_project_expr& x = exprs[e];
     if (!int_type(x.ret_type)) { g_err = "project: integer-typed expressions only"; return RW_ERR_UNSUPPORTED; }
+    if (!x.ops || x.n_ops < 1) { g_err = "project: malformed expression"; return RW_ERR_INVALID; }
+    std::vector<int> types;
+    for (int k = 0; k < x.n_ops; k++) {
+      const rw_expr_op& op = x.ops[k];
+      int t = 0, date = 0;
+      if (op.op == RW_EX_COL) {
+        if (op.arg < 0 || op.arg >= ch->n_cols || !int_type(ch->columns[op.arg].type)) { g_err = "project: operand column"; return RW_ERR_UNSUPPORTED; }
+        types.push_back(ch->columns[op.arg].type);
+      } else if (op.op == RW_EX_CONST) {
+        types.push_back(RW_T_INT64);
+      } else if (op.op == RW_EX_NEG || (op.op >= RW_EX_ADD && op.op <= RW_EX_TUMBLE_END)) {
+        t = op.arg == 0 ? RW_T_INT64 : op.arg;
+        if (t < RW_T_BOOL || t > RW_T_BYTEA) { g_err = "project: unknown result type of an operation"; return RW_ERR_INVALID; }
+        if (!int_type(t)) { g_err = "project: integer-typed operations only"; return RW_ERR_UNSUPPORTED; }
+        const size_t n_in = op.op == RW_EX_NEG ? 1 : 2;
+        if (types.size() < n_in) { g_err = "project: malformed expression"; return RW_ERR_INVALID; }
+        date = (op.op == RW_EX_TUMBLE_START || op.op == RW_EX_TUMBLE_END) && types[types.size() - n_in] == RW_T_DATE;
+        types.resize(types.size() - n_in);
+        types.push_back(t);
+      } else {
+        g_err = "project: unknown operation";
+        return RW_ERR_INVALID;
+      }
+      op_type[e].push_back(t);
+      op_date[e].push_back(date);
+    }
+    if (types.size() != 1) { g_err = "project: malformed expression"; return RW_ERR_INVALID; }
+  }
+  for (int e = 0; e < n_exprs; e++) {
+    const rw_project_expr& x = exprs[e];
     has_null[e] = 0;
     std::vector<uint64_t> valid((size_t)((n + 63) / 64), 0);
     const int w = type_width(x.ret_type);
@@ -1128,36 +1167,39 @@ extern "C" int32_t rwo_project(const rw_chunk* ch, const rw_project_expr* exprs,
       for (int k = 0; k < x.n_ops && ok; k++) {
         const rw_expr_op& op = x.ops[k];
         if (op.op == RW_EX_COL) {
-          if (op.arg < 0 || op.arg >= ch->n_cols || !int_type(ch->columns[op.arg].type)) { g_err = "project: operand column"; return RW_ERR_UNSUPPORTED; }
           Datum d = read_datum(ch->columns[op.arg], r);
           if (d.null) ok = false; else st.push_back(d.i);
         } else if (op.op == RW_EX_CONST) {
           st.push_back((i128)op.value);
-        } else if (op.op == RW_EX_NEG) {
-          if (st.empty()) { g_err = "project: malformed expression"; return RW_ERR_INVALID; }
-          st.back() = -st.back();
-          if (st.back() > (i128)INT64_MAX) ok = false;
         } else {
-          if (st.size() < 2) { g_err = "project: malformed expression"; return RW_ERR_INVALID; }
-          const i128 b = st.back();
-          st.pop_back();
-          const i128 a = st.back();
+          const i128 lo = type_min(op_type[e][k]), hi = -lo - 1;
           i128 v = 0;
-          switch (op.op) {
-            case RW_EX_ADD: v = a + b; break;
-            case RW_EX_SUB: v = a - b; break;
-            case RW_EX_MUL: v = a * b; break;
-            case RW_EX_DIV: if (b == 0) ok = false; else v = a / b; break;
-            case RW_EX_MOD: if (b == 0) ok = false; else v = a % b; break;
-            case RW_EX_TUMBLE_START: ok = window_start(a, b, &v); break;
-            case RW_EX_TUMBLE_END: ok = window_start(a, b, &v); v += b; break;
-            default: g_err = "project: unknown operation"; return RW_ERR_INVALID;
+          if (op.op == RW_EX_NEG) {
+            v = -st.back();
+          } else {
+            const i128 b = st.back();
+            st.pop_back();
+            i128 a = st.back();
+            switch (op.op) {
+              case RW_EX_ADD: v = a + b; break;
+              case RW_EX_SUB: v = a - b; break;
+              case RW_EX_MUL: v = a * b; break;
+              case RW_EX_DIV: if (b == 0) ok = false; else v = a / b; break;
+              case RW_EX_MOD: if (b == 0 || (a == lo && b == -1)) ok = false; else v = a % b; break;
+              default:  // RW_EX_TUMBLE_START / RW_EX_TUMBLE_END
+                if (op_date[e][k]) {  // days -> the microseconds of that midnight, checked at i64
+                  a *= (i128)86400000000LL;
+                  if (a > (i128)INT64_MAX || a < (i128)INT64_MIN) ok = false;
+                }
+                ok = ok && window_start(a, b, &v);
+                if (op.op == RW_EX_TUMBLE_END) v += b;
+                break;
+            }
           }
-          if (v > (i128)INT64_MAX || v < (i128)INT64_MIN) ok = false;  // checked i64 arithmetic
+          if (v > hi || v < lo) ok = false;  // checked at the operation's own result type
           st.back() = v;
         }
       }
-      if (ok && st.size() != 1) { g_err = "project: malformed expression"; return RW_ERR_INVALID; }
       int64_t v = ok ? (int64_t)st[0] : 0;
       if (ok && w == 4 && (v < INT32_MIN || v > INT32_MAX)) { ok = false; v = 0; }
       if (ok && w == 2 && (v < INT16_MIN || v > INT16_MAX)) { ok = false; v = 0; }

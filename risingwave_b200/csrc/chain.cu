@@ -138,11 +138,17 @@ static int filter_launch(const FilterPlanDev& p, const DevChunk& ch, uint8_t* ou
 // division by zero -- yields NULL, as does a NULL operand.  Ops and visibility pass through.  Offloaded expression
 // class: integer arithmetic in postfix form over integer-typed columns and constants (add / subtract / multiply /
 // divide / modulus / neg, src/expr/impl/src/scalar/arithmetic_op.rs `general_*` = checked ops) and tumble_start /
-// tumble_end over a microsecond interval (src/expr/impl/src/scalar/tumble.rs:91-112).  One thread per row and
-// expression, an 8-deep value stack in registers.  Roofline: HBM, the referenced columns in, one column out.
+// tumble_end over a microsecond interval (src/expr/impl/src/scalar/tumble.rs:91-112).  Every operation is checked at
+// its own result type (rw_expr_op.arg), as each checked_* of the reference is an op of that Rust integer type.  One
+// thread per row and expression, an 8-deep value stack in registers.  Roofline: HBM, the referenced columns in, one
+// column out.
 #define PROJ_MAX_EXPRS 16
 #define PROJ_MAX_OPS 24
 #define PROJ_STACK 8
+#define PROJ_US_PER_DAY 86400000000LL
+// ops[e][k] as the plan lowers it.  RW_EX_COL / RW_EX_CONST: as passed.  An operator: `value` = MIN of its result type
+// (the result must lie in [value, ~value]; a % -1 of value is NULL), `arg` = 1 when its first operand is a DATE (days)
+// that tumble_* turns into microseconds first, else 0.
 struct ProjectPlanDev {
   int n_exprs;
   int n_ops[PROJ_MAX_EXPRS];
@@ -195,24 +201,27 @@ __global__ void __launch_bounds__(256) project_kernel(ProjectPlanDev p, DevChunk
           else st[sp++] = load_i64(c, r);
         } else if (op.op == RW_EX_CONST) {
           st[sp++] = op.value;
-        } else if (op.op == RW_EX_NEG) {
-          if (st[sp - 1] == INT64_MIN) ok = false; else st[sp - 1] = -st[sp - 1];
         } else {
-          const long long b = st[--sp], a = st[sp - 1];
           long long v = 0;
-          switch (op.op) {
-            case RW_EX_ADD: ok = !add_ovf(a, b, &v); break;
-            case RW_EX_SUB: ok = !sub_ovf(a, b, &v); break;
-            case RW_EX_MUL: ok = !mul_ovf(a, b, &v); break;
-            case RW_EX_DIV: ok = b != 0 && !(a == INT64_MIN && b == -1); if (ok) v = a / b; break;
-            case RW_EX_MOD: ok = b != 0; if (ok) v = (b == -1) ? 0 : a % b; break;
-            case RW_EX_TUMBLE_START: ok = tumble_window_start(a, b, &v); break;
-            default: {  // RW_EX_TUMBLE_END = window start + window size
-              long long s0;
-              ok = tumble_window_start(a, b, &s0) && !add_ovf(s0, b, &v);
-              break;
+          if (op.op == RW_EX_NEG) {
+            ok = !sub_ovf(0, st[sp - 1], &v);
+          } else {
+            const long long b = st[--sp];
+            long long a = st[sp - 1];
+            switch (op.op) {
+              case RW_EX_ADD: ok = !add_ovf(a, b, &v); break;
+              case RW_EX_SUB: ok = !sub_ovf(a, b, &v); break;
+              case RW_EX_MUL: ok = !mul_ovf(a, b, &v); break;
+              case RW_EX_DIV: ok = b != 0 && !(a == INT64_MIN && b == -1); if (ok) v = a / b; break;
+              // checked_rem is None for MIN % -1 of the op's type (the quotient overflows), whatever the range check says
+              case RW_EX_MOD: ok = b != 0 && !(a == op.value && b == -1); if (ok) v = (b == -1) ? 0 : a % b; break;
+              default:  // RW_EX_TUMBLE_START / RW_EX_TUMBLE_END (= window start + window size)
+                if (op.arg) ok = !mul_ovf(a, PROJ_US_PER_DAY, &a);  // a DATE is the timestamp of its midnight (tumble.rs:34-37)
+                ok = ok && tumble_window_start(a, b, &v) && (op.op == RW_EX_TUMBLE_START || !add_ovf(v, b, &v));
+                break;
             }
           }
+          if (v < op.value || v > ~op.value) ok = false;  // outside the operation's own result type
           st[sp - 1] = v;
         }
       }
@@ -250,20 +259,27 @@ static int project_plan(const rw_chunk* c, const rw_project_expr* exprs, int32_t
     if (!proj_int_type(x.ret_type)) return fail(RW_ERR_UNSUPPORTED, "project: only integer-typed expressions are evaluated on the device");
     p->n_ops[e] = x.n_ops;
     p->ret_width[e] = type_width(x.ret_type);
+    int types[PROJ_MAX_OPS];  // RW_T_* of each stack slot: which tumble operand is a DATE is known here, not per row
     int depth = 0;
     for (int k = 0; k < x.n_ops; k++) {
-      const rw_expr_op& op = x.ops[k];
+      rw_expr_op op = x.ops[k];
       if (op.op == RW_EX_COL) {
         if (op.arg < 0 || op.arg >= c->n_cols || !proj_int_type(c->columns[op.arg].type))
           return fail(RW_ERR_UNSUPPORTED, "project: operand column must be integer-typed");
-        depth++;
+        types[depth++] = c->columns[op.arg].type;
       } else if (op.op == RW_EX_CONST) {
-        depth++;
-      } else if (op.op == RW_EX_NEG) {
-        if (depth < 1) return fail(RW_ERR_INVALID, "project: malformed postfix expression");
-      } else if (op.op >= RW_EX_ADD && op.op <= RW_EX_TUMBLE_END) {
-        if (depth < 2) return fail(RW_ERR_INVALID, "project: malformed postfix expression");
-        depth--;
+        types[depth++] = RW_T_INT64;
+      } else if (op.op == RW_EX_NEG || (op.op >= RW_EX_ADD && op.op <= RW_EX_TUMBLE_END)) {
+        const int t = op.arg == 0 ? RW_T_INT64 : op.arg;  // 0: INT64, the meaning of programs that predate typed ops
+        if (t < RW_T_BOOL || t > RW_T_BYTEA) return fail(RW_ERR_INVALID, "project: unknown result type of an operation");
+        if (!proj_int_type(t)) return fail(RW_ERR_UNSUPPORTED, "project: only integer-typed operations are evaluated on the device");
+        const int n_in = op.op == RW_EX_NEG ? 1 : 2;
+        if (depth < n_in) return fail(RW_ERR_INVALID, "project: malformed postfix expression");
+        depth -= n_in;
+        const int w = type_width(t);
+        op.value = w == 2 ? (int64_t)INT16_MIN : w == 4 ? (int64_t)INT32_MIN : INT64_MIN;
+        op.arg = (op.op == RW_EX_TUMBLE_START || op.op == RW_EX_TUMBLE_END) && types[depth] == RW_T_DATE;
+        types[depth++] = t;
       } else {
         return fail(RW_ERR_INVALID, "project: unknown operation");
       }

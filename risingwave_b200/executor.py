@@ -634,11 +634,12 @@ def parse_project_expr(text: str) -> Tuple[List[Tuple[int, int, int]], int]:
             if ty not in _EX_TYPES:
                 raise ValueError(f"unsupported expression type in {text!r}")
             prog = [op for a in args for op in a[0]]
+            # an operator's `arg` is its own result type: each checked op overflows at that width (rwgpu.h)
             if name == "neg" and len(args) == 1:
-                return prog + [(abi.EX_NEG, 0, 0)], _EX_TYPES[ty]
+                return prog + [(abi.EX_NEG, _EX_TYPES[ty], 0)], _EX_TYPES[ty]
             if name not in _EX_BIN or len(args) != 2:
                 raise ValueError(f"unsupported expression {name!r} in {text!r}")
-            return prog + [(_EX_BIN[name], 0, 0)], _EX_TYPES[ty]
+            return prog + [(_EX_BIN[name], _EX_TYPES[ty], 0)], _EX_TYPES[ty]
         val, ty = t.rsplit(":", 1)
         if ty not in _EX_TYPES:
             raise ValueError(f"unsupported expression type in {text!r}")

@@ -1,12 +1,12 @@
 """GPU: the device Filter (csrc/chain.cu, through the C ABI) vs the reference's golden vectors and the CPU oracle,
-and a join -> filter -> agg chain that never leaves the device."""
+and a join -> filter -> project -> agg chain that never leaves the device."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
 from risingwave_b200 import abi
-from risingwave_b200.executor import AggCall, FilterExecutor, HashAggExecutor, HashJoinExecutor, JoinParams, MockSource, parse_filter_expr
+from risingwave_b200.executor import AggCall, FilterExecutor, HashAggExecutor, HashJoinExecutor, JoinParams, MockSource, ProjectExecutor, parse_filter_expr
 from risingwave_b200.stream_chunk import Column, StreamChunk, net_multiset
 
 from helpers import load_golden, run_nexmark_q4, run_nexmark_q7, run_nexmark_q8
@@ -69,9 +69,11 @@ def test_filter_random_vs_oracle(cuda, oracle, expr, types, upsert):
 
 def test_join_filter_agg_chain_on_device(cuda, oracle):
     """q4-shaped chain: bid JOIN auction ON auction = id -> WHERE bid.date_time BETWEEN auction.date_time AND
-    auction.expires -> max(price), count(*) GROUP BY auction.  On the GPU the join output view feeds the filter
-    kernel and the agg push without leaving HBM (Project = re-ordered column pointers); the oracle runs the same
-    three operators on the host.  Compared: the agg deltas of every barrier (net multiset)."""
+    auction.expires -> Project(auction, tumble_start(bid.date_time, 250), price * 908 / 1000) -> max(price * 908 / 1000),
+    count(*) GROUP BY auction, window.  On the GPU the join output view feeds the filter kernel, rwgpu_project_device
+    (the auction column by pointer, the two computed columns by the project kernel) and the agg push without leaving
+    HBM; the oracle runs the same four operators on the host.  A wrong window or price changes the compared deltas:
+    the agg deltas of every barrier (net multiset)."""
     import torch
     from risingwave_b200 import device
     rng = np.random.default_rng(8)
@@ -83,7 +85,8 @@ def test_join_filter_agg_chain_on_device(cuda, oracle):
            rng.integers(0, 1500, n_bid).astype(np.int64), rng.integers(1, 10 ** 6, n_bid).astype(np.int64)]  # date_time, price
     # join output: bid cols 0..3 then auction cols 4..7
     expr = "(and:boolean (greater_than_or_equal:boolean $2:int8 $5:int8) (less_than_or_equal:boolean $2:int8 $6:int8))"
-    calls = [AggCall.from_pretty(c) for c in ("(count:int8)", "(max:int8 $1:int8)")]   # over the projected (auction, price)
+    calls = [AggCall.from_pretty(c) for c in ("(count:int8)", "(max:int8 $2:int8)")]   # over the projected (auction, window, price')
+    proj_exprs = ["(tumble_start:int8 $2:int8 250:int8)", "(divide:int8 (multiply:int8 $3:int8 908:int8) 1000:int8)"]
 
     def make(be):
         _, sl = MockSource.channel()
@@ -91,13 +94,14 @@ def test_join_filter_agg_chain_on_device(cuda, oracle):
         j = HashJoinExecutor(be, abi.JOIN_INNER, sl.into_executor(T4, [1]), sr.into_executor(T4, [0]), JoinParams([0], [1]),
                              JoinParams([0], []), [False], capacity_hint=n_auc)
         _, sa = MockSource.channel()
-        a = HashAggExecutor(be, sa.into_executor([abi.T_INT64, abi.T_INT64], []), True, calls, 0, [0], group_capacity_hint=n_auc)
+        a = HashAggExecutor(be, sa.into_executor([abi.T_INT64] * 3, []), True, calls, 0, [0, 1], group_capacity_hint=4 * n_auc)
         return j, a
 
     jo, ao = make(oracle)
     jg, ag = make(cuda)
     _, fsrc = MockSource.channel()
     fo = FilterExecutor(oracle, fsrc.into_executor(T4 + T4, []), expr)
+    po, pg = (ProjectExecutor(be, MockSource.channel()[1].into_executor(T4 + T4, []), proj_exprs) for be in (oracle, cuda))
     terms_py = parse_filter_expr(expr)
     terms = (abi.RwFilterTerm * len(terms_py))()
     for k, (cmp, lhs, rhs, const) in enumerate(terms_py):
@@ -110,11 +114,12 @@ def test_join_filter_agg_chain_on_device(cuda, oracle):
     B = 5000
     for e, lo in enumerate(range(0, n_bid, B)):
         part = [c[lo:lo + B] for c in bid]
-        # ---- oracle: join -> filter -> project (auction id, price) -> agg
+        # ---- oracle: join -> filter -> project (auction id, window, price') -> agg
         for ch in jo.eq_join_oneside(0, ins(part)):
             f = fo.filter(ch)
             if f is not None:
-                ao.apply_chunk(StreamChunk(f.ops, [f.columns[0], f.columns[3]], f.vis))
+                p = po.apply_project_exprs(f)
+                ao.apply_chunk(StreamChunk(f.ops, [f.columns[0]] + p.columns, f.vis))
         want = net_multiset(ao.flush_data(e + 1))
         # ---- GPU: everything stays in HBM
         view = device.join_push_device(jg, abi.SIDE_LEFT, dev(part))
@@ -124,11 +129,20 @@ def test_join_filter_agg_chain_on_device(cuda, oracle):
             cols[k].type, cols[k].data, cols[k].validity = view.col_types[k], view.col_ptrs[k], view.valid_ptrs[k]
         raw.n_rows, raw.n_cols, raw.ops, raw.visibility, raw.columns = view.n_rows, view.n_cols, view.ops_ptr, view.vis_ptr, cols
         f_ops, f_vis, f_n = device.filter_device(raw, view.n_rows, terms)
+        raw.ops, raw.visibility = f_ops.data_ptr(), f_vis.data_ptr()
+        n = max(view.n_rows, 1)
+        pdata = [torch.empty(n, dtype=torch.int64, device="cuda") for _ in proj_exprs]
+        pvalid = [torch.empty(n, dtype=torch.uint8, device="cuda") for _ in proj_exprs]
+        pnull = torch.zeros(len(proj_exprs), dtype=torch.int32, device="cuda")
+        device._check(device._lib().rwgpu_project_device(C.byref(raw), pg._exprs, len(proj_exprs), (C.c_void_p * 2)(*[d.data_ptr() for d in pdata]),
+                                                         (C.c_void_p * 2)(*[v.data_ptr() for v in pvalid]), C.c_void_p(pnull.data_ptr()), None))
+        assert int(pnull.sum().item()) == 0  # non-negative times and prices: neither window nor price' is NULL
         proj = abi.RwChunk()
-        pcols = (abi.RwColumn * 2)()
-        for k, src in enumerate((0, 3)):
-            pcols[k].type, pcols[k].data, pcols[k].validity = view.col_types[src], view.col_ptrs[src], view.valid_ptrs[src]
-        proj.n_rows, proj.n_cols, proj.ops, proj.visibility, proj.columns = view.n_rows, 2, f_ops.data_ptr(), f_vis.data_ptr(), pcols
+        pcols = (abi.RwColumn * 3)()
+        pcols[0].type, pcols[0].data, pcols[0].validity = view.col_types[0], view.col_ptrs[0], view.valid_ptrs[0]
+        for k, d in enumerate(pdata):
+            pcols[k + 1].type, pcols[k + 1].data, pcols[k + 1].validity = abi.T_INT64, d.data_ptr(), None
+        proj.n_rows, proj.n_cols, proj.ops, proj.visibility, proj.columns = view.n_rows, 3, f_ops.data_ptr(), f_vis.data_ptr(), pcols
         if int(f_n.item()) > 0:
             device._check(device._lib().rwgpu_agg_push_device(ag._h, C.byref(proj), None))
         got = net_multiset(ag.flush_data(e + 1))

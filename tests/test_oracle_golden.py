@@ -215,9 +215,10 @@ def test_project_golden(oracle, kat):
     run_project_kat(oracle, kat)
 
 
-def test_project_arithmetic_is_non_strict_and_tumble_follows_the_reference_formula(oracle):
-    """eval_infallible (project_scalar.rs:98): overflow / division by zero / NULL operand -> NULL for that row only;
-    tumble_start = ts - (r < 0 ? r + w : r), r = ts rem w (tumble.rs:96-111), checked against a Python restatement"""
+def test_project_arithmetic_is_non_strict_with_checked_rem_and_tumble_follows_the_reference_formula(oracle):
+    """eval_infallible (project_scalar.rs:98): overflow / division by zero / MIN % -1 (checked_rem, arithmetic_op.rs:98-107)
+    / NULL operand -> NULL for that row only; tumble_start = ts - (r < 0 ? r + w : r), r = ts rem w (tumble.rs:96-111),
+    checked against a Python restatement"""
     from risingwave_b200.executor import ProjectExecutor
     types = [abi.T_INT64, abi.T_INT64, abi.T_INT32]
     _, src = MockSource.channel()
@@ -254,7 +255,7 @@ def test_project_arithmetic_is_non_strict_and_tumble_follows_the_reference_formu
             if w is not None:
                 s0 = win(v, w)
                 want[2] = None if s0 is None else i64(s0 + w)
-                want[3] = None if w == 0 else v - trunc_div(v, w) * w
+                want[3] = None if w == 0 or (v == -big - 1 and w == -1) else v - trunc_div(v, w) * w  # checked_rem
             if x is not None:
                 d = x - v
                 want[4] = d if -(1 << 31) <= d < (1 << 31) else None
