@@ -312,6 +312,24 @@ struct AggOracle {
 
 const i128 DEC_MAX = (((i128)1) << 96) - 1;  // rust_decimal 96-bit mantissa
 
+// the signatures general.rs declares over the types of rwgpu.h: sum :18-27 (sum(int2 / int4) -> int8, sum(int8) ->
+// decimal, the internal sum(int8) -> int8 and sum0(int8) -> int8, sum(float4 / float8 / decimal) -> the same type),
+// min / max(any type but boolean) -> the argument type :93-128, count() / count(any) -> int8 :155-162
+bool agg_signature_ok(int kind, bool has_arg, int at, int ret) {
+  switch (kind) {
+    case RW_AGG_COUNT: return ret == RW_T_INT64;
+    case RW_AGG_SUM0: return has_arg && at == RW_T_INT64 && ret == RW_T_INT64;
+    case RW_AGG_SUM:
+      if (!has_arg) return false;
+      if (at == RW_T_INT16 || at == RW_T_INT32) return ret == RW_T_INT64;
+      if (at == RW_T_INT64) return ret == RW_T_INT64 || ret == RW_T_DECIMAL;
+      return (at == RW_T_FLOAT32 || at == RW_T_FLOAT64 || at == RW_T_DECIMAL) && ret == at;
+    case RW_AGG_MIN:
+    case RW_AGG_MAX: return has_arg && at != RW_T_BOOL && ret == at;
+    default: return true;
+  }
+}
+
 // one visible row into one call state: generated `update` wrapper src/expr/macro/src/gen.rs:838-912
 // + sum/min/max/count bodies src/expr/impl/src/aggregate/general.rs:28-41,104,123,155-162
 int agg_apply(const AggOracle& a, const rw_agg_call& c, Datum& st, const Datum& v, int arg_type, uint8_t op) {
@@ -350,8 +368,10 @@ int agg_apply(const AggOracle& a, const rw_agg_call& c, Datum& st, const Datum& 
       if (!a.append_only) return fail(RW_ERR_CUDA, "internal: retractable min/max goes through agg_apply_minput");
       if (op != RW_OP_INSERT) return fail(RW_ERR_INCONSISTENT, "attempt to retract on append-only min/max");
       if (st.null) { st = v; return RW_OK; }  // state = "ref": first value
+      // state.min(input) / state.max(input) (general.rs:104,123): Ord::min returns `self` and Ord::max `other` when the
+      // two compare equal, so on a tie (+0 / -0, two NaNs) min keeps the state and max takes the input
       int cmp = datum_cmp_nonnull(v, st, arg_type);
-      if ((c.kind == RW_AGG_MIN && cmp < 0) || (c.kind == RW_AGG_MAX && cmp > 0)) st = v;
+      if ((c.kind == RW_AGG_MIN && cmp < 0) || (c.kind == RW_AGG_MAX && cmp >= 0)) st = v;
       return RW_OK;
     }
   }
@@ -425,6 +445,15 @@ int32_t rwo_agg_create(const rw_agg_desc* d, rwo_agg** out) {
   a.in_types.assign(d->input_types, d->input_types + d->n_input_cols);
   a.key_idx.assign(d->group_key_indices, d->group_key_indices + d->n_group_keys);
   a.calls.assign(d->calls, d->calls + d->n_calls);
+  for (const rw_agg_call& c : a.calls) {
+    const int at = c.arg_col >= 0 && c.arg_col < d->n_input_cols ? a.in_types[c.arg_col] : 0;
+    if (c.arg_col >= d->n_input_cols) { delete h; return fail(RW_ERR_INVALID, "agg arg index"); }
+    if (!agg_signature_ok(c.kind, c.arg_col >= 0, at, c.ret_type)) {
+      delete h;
+      return fail(RW_ERR_INVALID, "aggregate signature not defined by the reference (general.rs)");
+    }
+    if (c.kind < RW_AGG_COUNT || c.kind > RW_AGG_SUM0 || is_varlen(at)) { delete h; return fail(RW_ERR_UNSUPPORTED, "agg kind / argument type"); }
+  }
   a.row_count_index = d->row_count_index;
   a.append_only = d->is_append_only != 0;
   a.strict = d->strict_consistency != 0;

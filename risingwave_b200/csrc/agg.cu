@@ -190,22 +190,30 @@ __device__ __forceinline__ void agg_apply_row(const AggTable& t, const AggPlanDe
     const int at = p.arg_type[c];
     const bool isf = (at == RW_T_FLOAT32 || at == RW_T_FLOAT64);
     if (kind == RW_AGG_SUM || kind == RW_AGG_SUM0) {
-      if (isf) {
+      if (at == RW_T_FLOAT32) {
+        // sum(float4) -> float4: an f32 state rounded after every add (general.rs:28-41 over F32), in the low half of
+        // the state word.  A CAS loop rather than atomicAdd(float*): atom.add.f32 flushes subnormals to zero.
+        const float x = ((const float*)ch.cols[ac].data)[r];
+        unsigned int* wp = (unsigned int*)sp;
+        unsigned int old = __ldcg(wp), seen;
+        do {
+          seen = old;
+          const float s = __uint_as_float(seen);
+          old = atomicCAS(wp, seen, __float_as_uint(retract ? __fsub_rn(s, x) : __fadd_rn(s, x)));
+        } while (old != seen);
+      } else if (isf) {
         double x = load_f64(ch.cols[ac], r);
         atomicAdd((double*)sp, retract ? -x : x);
       } else {
+        // exact 128-bit accumulation for every integer width: lo word here, carries into the cold hi word; the state
+        // is range-checked against its return type at the barrier (call_output)
         int64_t x = load_i64(ch.cols[ac], r);
         unsigned long long add = retract ? (0ull - (unsigned long long)x) : (unsigned long long)x;
-        if (ch.cols[ac].width == 8) {
-          // exact 128-bit accumulation: lo word here, carries into the cold hi word
-          bool neg = retract ? (x > 0) : (x < 0);
-          unsigned long long old = atomicAdd(sp, add);
-          unsigned long long nw = old + add;
-          long long hd = (neg ? -1ll : 0ll) + ((nw < old) ? 1ll : 0ll);
-          if (hd != 0) atomicAdd((unsigned long long*)(cold + p.hi_off[c]), (unsigned long long)hd);
-        } else {
-          atomicAdd(sp, add);  // |x| < 2^31: cannot leave int64 below 2^32 rows per group
-        }
+        bool neg = retract ? (x > 0) : (x < 0);
+        unsigned long long old = atomicAdd(sp, add);
+        unsigned long long nw = old + add;
+        long long hd = (neg ? -1ll : 0ll) + ((nw < old) ? 1ll : 0ll);
+        if (hd != 0) atomicAdd((unsigned long long*)(cold + p.hi_off[c]), (unsigned long long)hd);
       }
     } else if (p.mm_off[c] >= 0) {  // retractable MIN / MAX: materialized input (minput.rs:172-182)
       if (retract) { setflags &= ~(1u << c); continue; }  // retractions are applied by agg_mm_delete_kernel after this kernel
@@ -463,14 +471,12 @@ __device__ __forceinline__ OutVal call_output(const AggTable& t, const AggPlanDe
   } else if (!((flags >> c) & 1)) {
     v.null = (kind != RW_AGG_SUM0);  // sum0: init_state = 0; others NULL until a non-NULL input
   } else if (kind == RW_AGG_SUM || kind == RW_AGG_SUM0) {
-    if (isf) {
+    if (at == RW_T_FLOAT32) {  // sum(float4) -> float4: the f32 state, widened exactly (store_word narrows it back)
+      v.lo = (uint64_t)__double_as_longlong((double)__uint_as_float((unsigned int)s));
+    } else if (isf) {
       v.lo = s;
-      if (p.ret_type[c] == RW_T_FLOAT32) {  // sum(float4) -> float4
-        float f = (float)__longlong_as_double((long long)s);
-        v.lo = (uint64_t)__double_as_longlong((double)f);
-      }
     } else {
-      const long long hi = (p.hi_off[c] >= 0) ? (long long)cold[p.hi_off[c]] : (((long long)s) >> 63);
+      const long long hi = (long long)cold[p.hi_off[c]];  // every integer sum has a carry word
       v.lo = s;
       v.hi = (uint64_t)hi;
       if (p.ret_type[c] == RW_T_DECIMAL) {  // rust_decimal: 96-bit mantissa
@@ -919,7 +925,9 @@ __global__ void __launch_bounds__(256) agg_restore_kernel(AggTable t, AggPlanDev
       if (kind == RW_AGG_COUNT) {
         hot[p.KW + c] = (uint64_t)load_i64(sc, r);
       } else if (kind == RW_AGG_SUM || kind == RW_AGG_SUM0) {
-        if (isf) {
+        if (at == RW_T_FLOAT32) {
+          hot[p.KW + c] = (uint64_t)__float_as_uint(((const float*)sc.data)[r]);  // f32 state (agg_apply_row)
+        } else if (isf) {
           hot[p.KW + c] = (uint64_t)__double_as_longlong(load_f64(sc, r));
         } else if (p.ret_type[c] == RW_T_DECIMAL) {
           const uint64_t* d = (const uint64_t*)sc.data + r * 2;
@@ -1139,6 +1147,24 @@ static int agg_ensure_capacity(rwgpu_agg* h, uint64_t incoming) {
   RW_CUDA(cudaMemcpy(sh, h->status.p, sizeof(AggStatus), cudaMemcpyDeviceToHost));
   h->groups_upper = sh->n_groups;
   return RW_OK;
+}
+
+// the signatures src/expr/impl/src/aggregate/general.rs declares over the types of rwgpu.h (sum :18-27, min / max
+// :93-128, count :155-162); any other (kind, argument, return type) is refused with RW_ERR_INVALID before it is asked
+// whether the device runs it.  Unknown kinds pass here and are refused as unsupported.
+static bool agg_signature_ok(int kind, bool has_arg, int at, int ret) {
+  switch (kind) {
+    case RW_AGG_COUNT: return ret == RW_T_INT64;  // count() / count(any) -> int8
+    case RW_AGG_SUM0: return has_arg && at == RW_T_INT64 && ret == RW_T_INT64;
+    case RW_AGG_SUM:
+      if (!has_arg) return false;
+      if (at == RW_T_INT16 || at == RW_T_INT32) return ret == RW_T_INT64;
+      if (at == RW_T_INT64) return ret == RW_T_INT64 || ret == RW_T_DECIMAL;
+      return (at == RW_T_FLOAT32 || at == RW_T_FLOAT64 || at == RW_T_DECIMAL) && ret == at;
+    case RW_AGG_MIN:
+    case RW_AGG_MAX: return has_arg && at != RW_T_BOOL && ret == at;  // `-> auto`; no min / max(boolean)
+    default: return true;
+  }
 }
 
 static bool chunk_fast_ok(const rwgpu_agg* h, const DevChunk& ch) {
@@ -1462,31 +1488,24 @@ int32_t rwgpu_agg_create(const rw_agg_desc* d, rwgpu_agg** out) {
       used[call.arg_col] = true;
     }
     p.arg_type[c] = at;
+    if (!agg_signature_ok(call.kind, call.arg_col >= 0, at, call.ret_type))
+      return fail(RW_ERR_INVALID, "aggregate signature not defined by the reference (general.rs)");
     if (type_is_varlen(at)) return fail(RW_ERR_UNSUPPORTED, "aggregates over varlen arguments stay on the CPU executor");
     switch (call.kind) {
       case RW_AGG_COUNT:
-        if (call.ret_type != RW_T_INT64) return fail(RW_ERR_INVALID, "count returns int8");
         if (call.arg_col >= 0) fast = false;
         break;
       case RW_AGG_SUM:
       case RW_AGG_SUM0:
-        if (call.arg_col < 0) return fail(RW_ERR_INVALID, "sum needs an argument");
-        if (at == RW_T_DECIMAL || at == RW_T_BOOL) return fail(RW_ERR_UNSUPPORTED, "sum over this type stays on the CPU executor");
-        if (type_is_float(at)) {
-          if (call.ret_type != at) return fail(RW_ERR_INVALID, "sum(float) returns the same float type");
-          fast = false;
-        } else {
-          if (call.ret_type != RW_T_INT64 && call.ret_type != RW_T_DECIMAL) return fail(RW_ERR_INVALID, "sum(int) returns int8 or decimal");
-          if (type_width(at) == 8) p.hi_off[c] = cw++;
-          if (call.ret_type == RW_T_DECIMAL) { p.prevhi_off[c] = cw++; fast = false; }
-          if (type_width(at) != 8) fast = false;
-        }
+        if (at == RW_T_DECIMAL) return fail(RW_ERR_UNSUPPORTED, "sum(decimal) stays on the CPU executor");
+        if (!type_is_float(at)) p.hi_off[c] = cw++;  // every integer sum: exact 128-bit state, range-checked at the barrier
+        if (call.ret_type == RW_T_DECIMAL) p.prevhi_off[c] = cw++;
+        if (at != RW_T_INT64 || call.ret_type != RW_T_INT64) fast = false;
         h->all_flag_mask |= 1u << c;
         break;
       case RW_AGG_MIN:
       case RW_AGG_MAX:
-        if (call.arg_col < 0 || at == RW_T_DECIMAL) return fail(RW_ERR_UNSUPPORTED, "min/max over this type");
-        if (call.ret_type != at) return fail(RW_ERR_INVALID, "min/max returns the argument type");
+        if (at == RW_T_DECIMAL) return fail(RW_ERR_UNSUPPORTED, "min/max(decimal) stays on the CPU executor");
         if (type_width(at) != 8 || type_is_float(at)) fast = false;
         if (!d->is_append_only) {
           // retractable min/max is a MaterializedInput state (agg_state.rs:49-56, minput.rs): the call's input values
