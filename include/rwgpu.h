@@ -202,8 +202,11 @@ int32_t rwgpu_agg_profile(rwgpu_agg* h, int32_t enable, double* kernel_ms, uint6
 #define RW_SIDE_RIGHT 1
 
 /* restricted non-equi condition: `concat_row[lhs] <cmp> concat_row[rhs]` over the
- * (left cols || right cols) row, both integer-typed; anything richer stays on the CPU
- * executor (hash_join.rs:1362-1384 evaluates a general expression).                           */
+ * (left cols || right cols) row, compared as integers: both operands int2 / int4 / int8 (mixed
+ * widths are fine), or both of one and the same other non-float, non-decimal, fixed-width type
+ * (date with date, timestamp with timestamp ...).  Anything else -- float, decimal or varlen
+ * operands, date against timestamp, bool against int -- makes create return RW_ERR_UNSUPPORTED
+ * and stays on the CPU executor (hash_join.rs:1362-1384 evaluates a general expression).      */
 #define RW_CMP_NONE 0
 #define RW_CMP_LT 1
 #define RW_CMP_LE 2

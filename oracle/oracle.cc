@@ -46,6 +46,7 @@ struct Datum {
   bool null = true;
   i128 i = 0;     // all integer-like types, sign-extended; decimal mantissa
   double f = 0;   // float32 / float64 (float32 kept exactly representable)
+  uint32_t f32 = 0;  // float32 read from a column: its bits, so that a copy leaves with them (see write_datum)
   std::string s;  // varchar / bytea (BytesArray, bytes_array.rs:30-34): payload only
 };
 
@@ -79,12 +80,24 @@ Datum read_datum(const rw_column& c, int64_t r) {
     case RW_T_BOOL: d.i = p[r] ? 1 : 0; break;
     case RW_T_INT16: { int16_t v; memcpy(&v, p + r * 2, 2); d.i = v; break; }
     case RW_T_INT32: case RW_T_DATE: { int32_t v; memcpy(&v, p + r * 4, 4); d.i = v; break; }
-    case RW_T_FLOAT32: { float v; memcpy(&v, p + r * 4, 4); d.f = v; break; }
+    case RW_T_FLOAT32: { float v; memcpy(&v, p + r * 4, 4); memcpy(&d.f32, &v, 4); d.f = v; break; }
     case RW_T_FLOAT64: { double v; memcpy(&v, p + r * 8, 8); d.f = v; break; }
     case RW_T_DECIMAL: { i128 v; memcpy(&v, p + r * 16, 16); d.i = v; break; }
     default: { int64_t v; memcpy(&v, p + r * 8, 8); d.i = v; break; }
   }
   return d;
+}
+
+// the float4 bits of d: those it was read with while d.f is still their widening (a copy), else d.f narrowed.  Widening
+// and narrowing back returns every f32 but a signalling NaN unchanged; that one comes back quiet.
+uint32_t f32_bits(const Datum& d) {
+  float v;
+  memcpy(&v, &d.f32, 4);
+  const double w = v;
+  if (memcmp(&w, &d.f, 8) != 0) v = (float)d.f;
+  uint32_t b;
+  memcpy(&b, &v, 4);
+  return b;
 }
 
 // OrderedFloat equality: NaN == NaN, -0 == +0 (src/common/src/types/ordered_float.rs)
@@ -190,7 +203,7 @@ void write_datum(OutCol& c, const Datum& d) {
     case RW_T_BOOL: p[0] = d.i ? 1 : 0; break;
     case RW_T_INT16: { int16_t v = (int16_t)d.i; memcpy(p, &v, 2); break; }
     case RW_T_INT32: case RW_T_DATE: { int32_t v = (int32_t)d.i; memcpy(p, &v, 4); break; }
-    case RW_T_FLOAT32: { float v = (float)d.f; memcpy(p, &v, 4); break; }
+    case RW_T_FLOAT32: { uint32_t v = f32_bits(d); memcpy(p, &v, 4); break; }
     case RW_T_FLOAT64: { double v = d.f; memcpy(p, &v, 8); break; }
     case RW_T_DECIMAL: { i128 v = d.i; memcpy(p, &v, 16); break; }
     default: { int64_t v = (int64_t)d.i; memcpy(p, &v, 8); break; }
@@ -728,6 +741,19 @@ int32_t rwo_join_create(const rw_join_desc* d, rwo_join** out) {
   j.side[1].start_pos = j.side[0].n_cols;
   j.null_safe.assign(d->null_safe, d->null_safe + d->n_keys);
   j.cond = d->cond;
+  if (j.cond.cmp != RW_CMP_NONE) {  // the one integer comparison the C ABI carries (rwgpu.h rw_join_cond)
+    const int tot = j.side[0].n_cols + j.side[1].n_cols;
+    if (j.cond.cmp < 0 || j.cond.cmp > RW_CMP_NE || j.cond.lhs < 0 || j.cond.lhs >= tot || j.cond.rhs < 0 || j.cond.rhs >= tot) {
+      delete h;
+      return fail(RW_ERR_INVALID, "join condition");
+    }
+    auto col_type = [&](int idx) { return idx < j.side[0].n_cols ? j.side[0].types[idx] : j.side[1].types[idx - j.side[0].n_cols]; };
+    auto is_int = [](int t) { return t == RW_T_INT16 || t == RW_T_INT32 || t == RW_T_INT64; };
+    const int tl = col_type(j.cond.lhs), tr = col_type(j.cond.rhs);
+    for (int t : {tl, tr})
+      if (is_float(t) || t == RW_T_DECIMAL || is_varlen(t)) { delete h; return fail(RW_ERR_UNSUPPORTED, "non-integer join condition"); }
+    if (tl != tr && !(is_int(tl) && is_int(tr))) { delete h; return fail(RW_ERR_UNSUPPORTED, "join condition over two different non-integer types"); }
+  }
   j.strict = d->strict_consistency != 0;
   j.chunk_size = (size_t)std::max(d->chunk_size > 0 ? d->chunk_size : 1024, 2);  // builder.rs:44-47
   j.append_only_optimize = d->is_append_only && j.side[0].pk_in_jk && j.side[1].pk_in_jk;  // :381

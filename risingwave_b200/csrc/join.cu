@@ -1188,6 +1188,12 @@ __device__ __forceinline__ bool out_rows_equal(const JoinOutDev& o, const JoinPl
     const int w = p->out_width[k];
     const uint8_t* x = (const uint8_t*)o.col[k] + a * w;
     const uint8_t* y = (const uint8_t*)o.col[k] + b * w;
+    if (p->out_type[k] == RW_T_FLOAT32 || p->out_type[k] == RW_T_FLOAT64) {  // Datum equality of OrderedFloat: -0 == +0, NaN == NaN
+      const double fx = w == 4 ? (double)*(const float*)x : *(const double*)x;
+      const double fy = w == 4 ? (double)*(const float*)y : *(const double*)y;
+      if (fx != fy && (fx == fx || fy == fy)) return false;
+      continue;
+    }
     if (p->out_type[k] == RW_T_VARCHAR || p->out_type[k] == RW_T_BYTEA) {  // handles: compare the bytes they name
       const uint64_t hx = *(const uint64_t*)x, hy = *(const uint64_t*)y;
       if (hx == hy) continue;
@@ -2444,10 +2450,18 @@ int32_t rwgpu_join_create(const rw_join_desc* d, rwgpu_join** out) {
     int tot = d->left.n_cols + d->right.n_cols;
     if (p.cond_cmp < 0 || p.cond_cmp > RW_CMP_NE || p.cond_lhs < 0 || p.cond_lhs >= tot || p.cond_rhs < 0 || p.cond_rhs >= tot)
       return fail(RW_ERR_INVALID, "join condition");
-    for (int idx : {p.cond_lhs, p.cond_rhs}) {
-      int t = idx < d->left.n_cols ? d->left.types[idx] : d->right.types[idx - d->left.n_cols];
+    int ty[2];
+    for (int i = 0; i < 2; i++) {
+      const int idx = i ? p.cond_rhs : p.cond_lhs;
+      const int t = idx < d->left.n_cols ? d->left.types[idx] : d->right.types[idx - d->left.n_cols];
       if (type_is_float(t) || t == RW_T_DECIMAL || type_is_varlen(t)) return fail(RW_ERR_UNSUPPORTED, "non-integer join condition stays on the CPU executor");
+      ty[i] = t;
     }
+    // cond_ok compares raw integers: int2 / int4 / int8 mix (the reference widens them), every other type only with itself
+    // (date against timestamp would compare days with microseconds; the reference casts the date first)
+    auto is_int = [](int t) { return t == RW_T_INT16 || t == RW_T_INT32 || t == RW_T_INT64; };
+    if (ty[0] != ty[1] && !(is_int(ty[0]) && is_int(ty[1])))
+      return fail(RW_ERR_UNSUPPORTED, "join condition over two different non-integer types stays on the CPU executor");
   }
   p.single_key = (p.n_keys == 1);
   p.KW = p.single_key ? 1 : 1 + p.n_keys;

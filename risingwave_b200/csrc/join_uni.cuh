@@ -712,14 +712,20 @@ __device__ __forceinline__ void uni_deferred_body(const JoinPlanDev* __restrict_
   if (!PROBE_ONLY && new_keys) atomicAdd(&st->n_keys[0], (unsigned long long)new_keys);
 }
 
-// pk equality of a stored row (columns c[], null mask) with chunk row r
+// pk equality of a stored row (columns c[], null mask) with chunk row r; a float8 pk column compares by the class
+// load_key_word gives it (-0 == +0, one NaN), as pk_equal of the other paths does
 __device__ __forceinline__ bool uni_pk_equal(const JoinPlanDev* p, int S, const uint64_t* c, uint32_t nmask, const DevChunk& ch, int64_t r) {
   for (int i = 0; i < p->n_pk[S]; i++) {
     const int k = p->pk_col[S][i];
     const bool n1 = (nmask >> k) & 1u, n2 = col_is_null(ch.cols[k], r);
     if (n1 != n2) return false;
     if (n1) continue;
-    if (c[k] != ((const uint64_t*)ch.cols[k].data)[r]) return false;
+    const uint64_t x = c[k], y = ((const uint64_t*)ch.cols[k].data)[r];
+    if (x != y) {
+      if (p->col_type[S][k] != RW_T_FLOAT64) return false;
+      const double fx = __longlong_as_double((long long)x), fy = __longlong_as_double((long long)y);
+      if (fx != fy && (fx == fx || fy == fy)) return false;
+    }
   }
   return true;
 }
