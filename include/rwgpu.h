@@ -341,7 +341,11 @@ int32_t rwgpu_join_profile(rwgpu_join* h, int32_t enable, double* kernel_ms, uin
 /* HOST: vnode per row (invisible rows still get a value, as in the reference).               */
 int32_t rwgpu_vnode_compute(const rw_chunk* chunk, const int32_t* key_indices, int32_t n_keys,
                             int32_t vnode_count, uint16_t* out_vnodes);
-/* HOST: the op rewrite of dispatch.rs:1001-1019 (U-/U+ whose dist key changed -> -/+).       */
+/* HOST: the op rewrite of dispatch.rs:976-1023 (U-/U+ whose dist key changed -> -/+).  Over the visible rows, a U+
+ * pairs with the last U- that no earlier U+ has taken, whatever + / - rows lie between them; a U- that a later U-
+ * replaces before any U+ keeps its op.  The key compares as a Datum (NULL == NULL, -0 == +0, every NaN equal).
+ * RW_ERR_INCONSISTENT: a U+ with no U- to take ("missing U- before U+"), or a U- that no U+ follows anywhere in the
+ * chunk ("missing U+ after U-").  Invisible rows keep their op.  Key arguments as for rwgpu_vnode_compute.      */
 int32_t rwgpu_dispatch_rewrite_ops(const rw_chunk* chunk, const int32_t* key_indices, int32_t n_keys,
                                    uint8_t* out_ops);
 /* DEVICE: partition the visible rows of a device chunk by destination

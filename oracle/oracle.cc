@@ -970,9 +970,23 @@ static uint16_t vnode_from_row_id(int64_t id, int vnode_count) {
   return (uint16_t)(part % (uint64_t)vnode_count);
 }
 
+// the arguments the device's make_vnode_plan (csrc/shuffle.cu) accepts, refused with the same status codes
+static int vnode_args(const rw_chunk* ch, const int32_t* keys, int32_t n_keys, int32_t vnode_count) {
+  if (n_keys < 1 || n_keys > 8) return fail(RW_ERR_UNSUPPORTED, "1..8 distribution key columns");
+  if (vnode_count < 1 || vnode_count > 32768) return fail(RW_ERR_INVALID, "vnode_count (vnode.rs:79 MAX_COUNT = 2^15)");
+  for (int k = 0; k < ch->n_cols; k++)
+    if (is_varlen(ch->columns[k].type)) return fail(RW_ERR_UNSUPPORTED, "the hash shuffle does not carry varlen columns");
+  for (int k = 0; k < n_keys; k++)
+    if (keys[k] < 0 || keys[k] >= ch->n_cols) return fail(RW_ERR_INVALID, "key index");
+  return RW_OK;
+}
+
 // VirtualNode::compute_chunk (src/common/src/hash/consistent_hash/vnode.rs:151-182);
 // get_hash_values hashes only VISIBLE rows (data_chunk.rs:338-355) => invisible rows: crc32("")=0
 int32_t rwo_vnode_compute(const rw_chunk* ch, const int32_t* keys, int32_t n_keys, int32_t vnode_count, uint16_t* out) {
+  if (!ch || !keys || !out) return fail(RW_ERR_INVALID, "null");
+  int rc = vnode_args(ch, keys, n_keys, vnode_count);
+  if (rc != RW_OK) return rc;
   if (n_keys == 1 && ch->columns[keys[0]].type == RW_T_SERIAL) {
     const rw_column& c = ch->columns[keys[0]];
     for (int64_t r = 0; r < ch->n_rows; r++) {
@@ -996,8 +1010,13 @@ int32_t rwo_vnode_compute(const rw_chunk* ch, const int32_t* keys, int32_t n_key
   return RW_OK;
 }
 
-// the op rewrite of HashDataDispatcher::dispatch_data (src/stream/src/executor/dispatch.rs:985-1023)
+// the op rewrite of HashDataDispatcher::dispatch_data (src/stream/src/executor/dispatch.rs:976-1023): a visible U+
+// pairs with the last visible U- that no earlier U+ has taken (`last_update_delete_row_idx.take()`), whatever visible
+// +/- rows lie between them; a U- that a later U- replaces keeps its op
 int32_t rwo_dispatch_rewrite_ops(const rw_chunk* ch, const int32_t* keys, int32_t n_keys, uint8_t* out_ops) {
+  if (!ch || !keys || !out_ops) return fail(RW_ERR_INVALID, "null");
+  int rc = vnode_args(ch, keys, n_keys, 256);
+  if (rc != RW_OK) return rc;
   int64_t last_ud = -1;
   for (int64_t r = 0; r < ch->n_rows; r++) {
     uint8_t op = ch->ops[r];

@@ -115,16 +115,32 @@ __global__ void __launch_bounds__(256) vnode_kernel(DevChunk ch, VnodePlan p, ui
   }
 }
 
-// the op rewrite of dispatch.rs:1001-1019: a visible U+ looks back to the previous visible row (its U-)
+// the op rewrite of dispatch.rs:976-1023, one thread per row.  The reference pairs a visible U+ with the last visible U-
+// that no earlier U+ has taken (`last_update_delete_row_idx.take()`), whatever visible +/- rows lie between them:
+//  * a visible U+ walks back over the visible rows, skipping + / -, to the nearest U- and rewrites both rows; meeting a
+//    U+ or the chunk start first is "missing U- before U+" (bit 0 of *err);
+//  * a visible U- walks forward the same way: if it meets a U+, that U+ writes its op; if it meets another U-, which
+//    replaces it as the pending one, it keeps its op; if it meets the chunk end, it is "missing U+ after U-" (bit 1).
+__device__ __forceinline__ bool rewrite_skips(const DevChunk& ch, int64_t r) {
+  const uint8_t op = ch.ops[r];
+  return !row_visible(ch, r, op) || op == RW_OP_INSERT || op == RW_OP_DELETE;
+}
 __global__ void dispatch_rewrite_kernel(DevChunk ch, VnodePlan p, uint8_t* out_ops, unsigned int* err) {
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < ch.n; r += (int64_t)gridDim.x * blockDim.x) {
-    uint8_t op = ch.ops[r];
-    if (op != RW_OP_UPDATE_INSERT || !row_visible(ch, r, op)) {
-      if (op != RW_OP_UPDATE_DELETE || !row_visible(ch, r, op)) out_ops[r] = op;
+    const uint8_t op = ch.ops[r];
+    if (rewrite_skips(ch, r) || (op != RW_OP_UPDATE_INSERT && op != RW_OP_UPDATE_DELETE)) {
+      out_ops[r] = op;
+      continue;
+    }
+    if (op == RW_OP_UPDATE_DELETE) {
+      int64_t j = r + 1;
+      while (j < ch.n && rewrite_skips(ch, j)) j++;
+      if (j >= ch.n) atomicOr(err, 2u);
+      if (j >= ch.n || ch.ops[j] != RW_OP_UPDATE_INSERT) out_ops[r] = op;
       continue;
     }
     int64_t j = r - 1;
-    while (j >= 0 && !row_visible(ch, j, ch.ops[j])) j--;
+    while (j >= 0 && rewrite_skips(ch, j)) j--;
     if (j < 0 || ch.ops[j] != RW_OP_UPDATE_DELETE) { atomicOr(err, 1u); out_ops[r] = op; continue; }
     bool changed = false;
     for (int k = 0; k < p.n_keys; k++) {
@@ -140,16 +156,6 @@ __global__ void dispatch_rewrite_kernel(DevChunk ch, VnodePlan p, uint8_t* out_o
     }
     out_ops[j] = changed ? RW_OP_DELETE : RW_OP_UPDATE_DELETE;
     out_ops[r] = changed ? RW_OP_INSERT : RW_OP_UPDATE_INSERT;
-  }
-}
-// a visible U- with no following visible U+ keeps its op (and is an error in the reference)
-__global__ void dispatch_rewrite_fix_kernel(DevChunk ch, uint8_t* out_ops, unsigned int* err) {
-  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < ch.n; r += (int64_t)gridDim.x * blockDim.x) {
-    uint8_t op = ch.ops[r];
-    if (op != RW_OP_UPDATE_DELETE || !row_visible(ch, r, op)) continue;
-    int64_t j = r + 1;
-    while (j < ch.n && !row_visible(ch, j, ch.ops[j])) j++;
-    if (j >= ch.n || ch.ops[j] != RW_OP_UPDATE_INSERT) { atomicOr(err, 2u); out_ops[r] = op; }
   }
 }
 
@@ -789,7 +795,6 @@ int32_t rwgpu_dispatch_rewrite_ops(const rw_chunk* c, const int32_t* keys, int32
   unsigned int* err = (unsigned int*)(dout.as<uint8_t>() + ((size_t)c->n_rows + 7) / 8 * 8);
   RW_CUDA(cudaMemset(dout.p, 0, (size_t)c->n_rows + 16));
   dispatch_rewrite_kernel<<<grid_rows(c->n_rows, 256), 256>>>(ch, p, dout.as<uint8_t>(), err);
-  dispatch_rewrite_fix_kernel<<<grid_rows(c->n_rows, 256), 256>>>(ch, dout.as<uint8_t>(), err);
   RW_CUDA(cudaGetLastError());
   RW_CUDA(cudaMemcpy(out_ops, dout.p, (size_t)c->n_rows, cudaMemcpyDeviceToHost));
   unsigned int e = 0;

@@ -11,7 +11,7 @@ One process per GPU.  Per device batch:
 Row order per (source, key) is preserved, and a receiver concatenates sources in rank order, so
 per-key order is deterministic.  Barriers are a host-side `dist.barrier()` (they are broadcast in
 the reference too, dispatch.rs:940-947).  `U-/U+` pairs whose distribution key changes must be
-rewritten to `-/+` before partitioning (`rwgpu_dispatch_rewrite_ops`, dispatch.rs:1001-1019).
+rewritten to `-/+` before partitioning (`rwgpu_dispatch_rewrite_ops`, dispatch.rs:976-1023).
 
 The split-size logic is backend-agnostic (`plan_splits`) and is covered on CPU with gloo,
 world_size 2 (tests/test_exchange_gloo.py).
