@@ -206,7 +206,8 @@ int32_t rwgpu_agg_profile(rwgpu_agg* h, int32_t enable, double* kernel_ms, uint6
  * widths are fine), or both of one and the same other non-float, non-decimal, fixed-width type
  * (date with date, timestamp with timestamp ...).  Anything else -- float, decimal or varlen
  * operands, date against timestamp, bool against int -- makes create return RW_ERR_UNSUPPORTED
- * and stays on the CPU executor (hash_join.rs:1362-1384 evaluates a general expression).      */
+ * and stays on the CPU executor (hash_join.rs:1362-1384 evaluates a general expression).  Filter
+ * terms follow the same rule.                                                                   */
 #define RW_CMP_NONE 0
 #define RW_CMP_LT 1
 #define RW_CMP_LE 2
@@ -433,19 +434,27 @@ int32_t rwgpu_shuffle_exchange_flat_device(const rw_chunk* chunk, const int32_t*
 
 /* ================================================================ Filter (operator chaining on the device)
  * Replaces FilterExecutorInner::filter           src/stream/src/executor/filter.rs:58-150
- * for predicates that are a CONJUNCTION of integer comparisons `col cmp col` / `col cmp constant`
- * (Int16/32/64, Date, Time, Timestamptz, Serial, Bool).  A NULL operand makes its term NULL and
- * the row's result false (filter.rs:79 `res.unwrap_or(false)`); everything else the expression
- * framework can evaluate stays on the CPU FilterExecutor.  Project with InputRef expressions
- * (project_scalar.rs:100-120) is a re-ordering of column pointers in the caller and needs no kernel.
+ * for predicates that are a CONJUNCTION of integer comparisons `col cmp col` / `col cmp constant`,
+ * compared as raw integers under the operand rule of join conditions (above): int2 / int4 / int8
+ * mix, and bool, serial, date, time, timestamp and timestamptz compare only with themselves; a
+ * constant has the left operand's type.  Any other pair (date against timestamp, bool against int8,
+ * a float, decimal or varlen operand) is RW_ERR_UNSUPPORTED and stays on the CPU FilterExecutor, as
+ * does everything else the expression framework can evaluate.  A bad comparison or column index is
+ * RW_ERR_INVALID.  A NULL operand makes its term NULL and the row's result false (filter.rs:79
+ * `res.unwrap_or(false)`).  Project with InputRef expressions (project_scalar.rs:100-120) is a
+ * re-ordering of column pointers in the caller and needs no kernel.
  *
  * Output: out_ops[n_rows] and the packed visibility out_visibility[(n_rows+63)/64] of a chunk that
- * has the input's columns.  Rows that were invisible in the input stay invisible with their op
+ * has the input's columns; every word is written, the bits past n_rows zero.  Rows that were
+ * invisible in the input -- a cleared visibility bit or op 0 -- stay invisible with their op
  * unchanged (the reference compacts them away first, filter.rs:182); the visible rows carry exactly
- * the ops / visibility the reference produces, U-/U+ pairs included (filter.rs:107-141; a pair is a
- * visible U- and the next visible row, which must be U+).  upsert != 0 selects the UPSERT rules
- * (filter.rs:82-106).  *n_visible (may be NULL) receives the number of visible output rows
- * (0 => the reference yields no chunk, filter.rs:146-150).                                       */
+ * the ops / visibility the reference produces, U-/U+ pairs included (filter.rs:107-141).  A visible
+ * U- pairs with the next visible row only if that row is a U+; a U- or U+ without its partner (which
+ * well-formed streams never carry) is filtered like a - or + and keeps its op.  upsert != 0 selects
+ * the UPSERT rules (filter.rs:82-106).  *n_visible (may be NULL) receives the number of visible
+ * output rows (0 => the reference yields no chunk, filter.rs:146-150).  rwgpu_filter_device reads
+ * neighbouring rows' input ops and visibility while it writes: outputs that alias the chunk's ops
+ * or visibility are RW_ERR_INVALID.                                                               */
 typedef struct rw_filter_term {
   int32_t cmp;       /* RW_CMP_LT .. RW_CMP_NE                                  */
   int32_t lhs_col;

@@ -53,6 +53,18 @@ struct Datum {
 bool is_float(int t) { return t == RW_T_FLOAT32 || t == RW_T_FLOAT64; }
 bool is_varlen(int t) { return t == RW_T_VARCHAR || t == RW_T_BYTEA; }
 
+// which operand types a join condition or filter term compares as raw integers: int2 / int4 / int8 with each other (the
+// reference widens them, src/expr/impl/src/scalar/cmp.rs:44-51), any other orderable fixed-width type only with itself
+// (cmp.rs:24-160; date against timestamp, which the reference evaluates by casting the date, is not restated)
+bool cmp_operands_ok(int a, int b) {
+  auto is_int = [](int t) { return t == RW_T_INT16 || t == RW_T_INT32 || t == RW_T_INT64; };
+  auto ordered = [&](int t) {
+    return is_int(t) || t == RW_T_BOOL || t == RW_T_SERIAL || t == RW_T_DATE || t == RW_T_TIME || t == RW_T_TIMESTAMP ||
+           t == RW_T_TIMESTAMPTZ;
+  };
+  return ordered(a) && ordered(b) && (a == b || (is_int(a) && is_int(b)));
+}
+
 int type_width(int t) {
   switch (t) {
     case RW_T_BOOL: return 1;
@@ -748,11 +760,7 @@ int32_t rwo_join_create(const rw_join_desc* d, rwo_join** out) {
       return fail(RW_ERR_INVALID, "join condition");
     }
     auto col_type = [&](int idx) { return idx < j.side[0].n_cols ? j.side[0].types[idx] : j.side[1].types[idx - j.side[0].n_cols]; };
-    auto is_int = [](int t) { return t == RW_T_INT16 || t == RW_T_INT32 || t == RW_T_INT64; };
-    const int tl = col_type(j.cond.lhs), tr = col_type(j.cond.rhs);
-    for (int t : {tl, tr})
-      if (is_float(t) || t == RW_T_DECIMAL || is_varlen(t)) { delete h; return fail(RW_ERR_UNSUPPORTED, "non-integer join condition"); }
-    if (tl != tr && !(is_int(tl) && is_int(tr))) { delete h; return fail(RW_ERR_UNSUPPORTED, "join condition over two different non-integer types"); }
+    if (!cmp_operands_ok(col_type(j.cond.lhs), col_type(j.cond.rhs))) { delete h; return fail(RW_ERR_UNSUPPORTED, "join condition operand types"); }
   }
   j.strict = d->strict_consistency != 0;
   j.chunk_size = (size_t)std::max(d->chunk_size > 0 ? d->chunk_size : 1024, 2);  // builder.rs:44-47
@@ -1061,29 +1069,31 @@ int32_t rwo_eliminate_adjacent_noop_update(const rw_chunk* ch, uint8_t* out_ops,
 }  // extern "C"
 
 // FilterExecutorInner::filter (src/stream/src/executor/filter.rs:58-150), restated literally: the chunk is
-// compacted first (execute_inner, filter.rs:182), the predicate gives Option<bool> per row
-// (`res.unwrap_or(false)`, :79), then the op rules produce new ops / visibility for the compacted rows.
-// The results are scattered back to the positions of the input's visible rows (invisible input rows keep
-// their op and stay invisible) so that the signature equals rwgpu_filter's.
+// compacted first (execute_inner, filter.rs:182; a row with op 0 is invisible like a cleared visibility bit), the
+// predicate gives Option<bool> per row (`res.unwrap_or(false)`, :79), then the op rules produce new ops / visibility for
+// the compacted rows.  The results are scattered back to the positions of the input's visible rows (invisible input rows
+// keep their op, op 0 included, and stay invisible) so that the signature equals rwgpu_filter's.
 // Predicate = conjunction of integer comparisons with SQL three-valued logic: a NULL operand makes the
 // term NULL; AND of terms is NULL/false unless every term is true -> unwrap_or(false) == "all terms true".
+// The reference only sees U- immediately followed by U+ (stream_chunk.rs:40-42).  The project's rule for anything else
+// (the device's): a U- pairs with the next visible row only if that row is a U+, a U+ with the previous visible row only
+// if that row is a U-; an unpaired U- or U+ is filtered like a - or + and keeps its op.
 extern "C" int32_t rwo_filter(const rw_chunk* ch, const rw_filter_term* terms, int32_t n_terms, int32_t upsert, uint8_t* out_ops,
                               uint64_t* out_visibility, int64_t* n_visible) {
+  if (!ch || !terms || !out_ops || !out_visibility) return fail(RW_ERR_INVALID, "null");
   const int64_t n = ch->n_rows;
-  if (n_terms < 1 || n_terms > 8) { g_err = "filter: 1..8 conjuncts"; return RW_ERR_UNSUPPORTED; }
+  if (n_terms < 1 || n_terms > 8) return fail(RW_ERR_UNSUPPORTED, "filter: 1..8 conjuncts");
   for (int k = 0; k < n_terms; k++) {
-    auto ok = [&](int c) { return c >= 0 && c < ch->n_cols && !is_float(ch->columns[c].type) && ch->columns[c].type != RW_T_DECIMAL &&
-                                  ch->columns[c].type != RW_T_TIMESTAMP; };
-    if (terms[k].cmp < RW_CMP_LT || terms[k].cmp > RW_CMP_NE) { g_err = "filter: comparison"; return RW_ERR_INVALID; }
-    if (!ok(terms[k].lhs_col) || terms[k].rhs_col < -1 || (terms[k].rhs_col >= 0 && !ok(terms[k].rhs_col))) {
-      g_err = "filter: only integer-typed columns are compared";
-      return RW_ERR_UNSUPPORTED;
-    }
+    const rw_filter_term& t = terms[k];
+    if (t.cmp < RW_CMP_LT || t.cmp > RW_CMP_NE) return fail(RW_ERR_INVALID, "filter: comparison");
+    if (t.lhs_col < 0 || t.lhs_col >= ch->n_cols || t.rhs_col < -1 || t.rhs_col >= ch->n_cols) return fail(RW_ERR_INVALID, "filter: column index");
+    const int lt = ch->columns[t.lhs_col].type, rt = t.rhs_col >= 0 ? ch->columns[t.rhs_col].type : lt;  // a constant takes the lhs's type
+    if (!cmp_operands_ok(lt, rt)) return fail(RW_ERR_UNSUPPORTED, "filter: operand types");
   }
   // compact_vis
   std::vector<int64_t> pos;
   for (int64_t r = 0; r < n; r++)
-    if (bit_get(ch->visibility, r)) pos.push_back(r);
+    if (ch->ops[r] != 0 && bit_get(ch->visibility, r)) pos.push_back(r);
   // pred_output: Option<bool> per compacted row
   auto pred = [&](int64_t r) -> int {  // 1 true, 0 false, -1 NULL
     bool any_null = false, any_false = false;
@@ -1106,35 +1116,31 @@ extern "C" int32_t rwo_filter(const rw_chunk* ch, const rw_filter_term* terms, i
     }
     return any_false ? 0 : (any_null ? -1 : 1);
   };
-  std::vector<uint8_t> new_ops;
-  std::vector<bool> new_vis;
-  bool last_res = false;
-  for (size_t i = 0; i < pos.size(); i++) {
-    const uint8_t op = ch->ops[pos[i]];
+  const size_t m = pos.size();
+  std::vector<uint8_t> new_ops(m);
+  std::vector<bool> new_vis(m);
+  auto op_at = [&](size_t i) { return ch->ops[pos[i]]; };
+  for (size_t i = 0; i < m; i++) {
+    const uint8_t op = op_at(i);
     const bool res = pred(pos[i]) == 1;  // unwrap_or(false)
     if (upsert) {  // :82-106
-      if (op == RW_OP_INSERT || op == RW_OP_UPDATE_INSERT) { new_ops.push_back(res ? RW_OP_INSERT : RW_OP_DELETE); new_vis.push_back(true); }
-      else { new_ops.push_back(RW_OP_DELETE); new_vis.push_back(true); }
-    } else if (op == RW_OP_INSERT || op == RW_OP_DELETE) {  // :108-111
-      new_ops.push_back(op);
-      new_vis.push_back(res);
-    } else if (op == RW_OP_UPDATE_DELETE) {  // :112-114
-      last_res = res;
-    } else {  // UpdateInsert :115-141
-      if (last_res && !res) { new_ops.push_back(RW_OP_DELETE); new_ops.push_back(RW_OP_UPDATE_INSERT); new_vis.push_back(true); new_vis.push_back(false); }
-      else if (!last_res && res) { new_ops.push_back(RW_OP_UPDATE_DELETE); new_ops.push_back(RW_OP_INSERT); new_vis.push_back(false); new_vis.push_back(true); }
-      else if (last_res && res) { new_ops.push_back(RW_OP_UPDATE_DELETE); new_ops.push_back(RW_OP_UPDATE_INSERT); new_vis.push_back(true); new_vis.push_back(true); }
-      else { new_ops.push_back(RW_OP_UPDATE_DELETE); new_ops.push_back(RW_OP_UPDATE_INSERT); new_vis.push_back(false); new_vis.push_back(false); }
+      new_ops[i] = (op == RW_OP_INSERT || op == RW_OP_UPDATE_INSERT) && res ? RW_OP_INSERT : RW_OP_DELETE;
+      new_vis[i] = true;
+    } else if (op == RW_OP_UPDATE_DELETE && i + 1 < m && op_at(i + 1) == RW_OP_UPDATE_INSERT) {  // :112-141, one pair
+      const bool last_res = res, res2 = pred(pos[i + 1]) == 1;
+      if (last_res && !res2) { new_ops[i] = RW_OP_DELETE; new_ops[i + 1] = RW_OP_UPDATE_INSERT; new_vis[i] = true; new_vis[i + 1] = false; }
+      else if (!last_res && res2) { new_ops[i] = RW_OP_UPDATE_DELETE; new_ops[i + 1] = RW_OP_INSERT; new_vis[i] = false; new_vis[i + 1] = true; }
+      else { new_ops[i] = RW_OP_UPDATE_DELETE; new_ops[i + 1] = RW_OP_UPDATE_INSERT; new_vis[i] = new_vis[i + 1] = last_res; }
+      i++;
+    } else {  // + / - (:108-111), and an unpaired U- or U+ by the project's rule
+      new_ops[i] = op;
+      new_vis[i] = res;
     }
   }
-  if (new_ops.size() != pos.size()) {  // a U- without its U+ (StreamChunk::with_visibility would panic on the length)
-    g_err = "filter: UpdateDelete without a following UpdateInsert";
-    return RW_ERR_INCONSISTENT;
-  }
-  memcpy(out_ops, ch->ops, (size_t)n);
+  if (n) memcpy(out_ops, ch->ops, (size_t)n);
   memset(out_visibility, 0, (size_t)((n + 63) / 64) * 8);
   int64_t cnt = 0;
-  for (size_t i = 0; i < pos.size(); i++) {
+  for (size_t i = 0; i < m; i++) {
     out_ops[pos[i]] = new_ops[i];
     if (new_vis[i]) { out_visibility[pos[i] >> 6] |= 1ull << (pos[i] & 63); cnt++; }
   }

@@ -58,6 +58,20 @@ bool type_is_float(int t) { return t == RW_T_FLOAT32 || t == RW_T_FLOAT64; }
 bool type_is_varlen(int t) { return t == RW_T_VARCHAR || t == RW_T_BYTEA; }
 bool type_supported(int t) { return type_width(t) != 0; }
 
+// Join conditions and filter terms compare raw integers.  int2 / int4 / int8 mix (the reference widens them,
+// src/expr/impl/src/scalar/cmp.rs:44-51); every other type compares only with itself (cmp.rs:24-160 has no
+// bool / int8, time / int8 or serial / int8 function, and date against timestamp would compare days with
+// microseconds where the reference casts the date first).  Floats, decimals and varlen values are not compared.
+bool cmp_operands_ok(int a, int b) {
+  auto is_int = [](int t) { return t == RW_T_INT16 || t == RW_T_INT32 || t == RW_T_INT64; };
+  auto is_ordered = [&](int t) {
+    return is_int(t) || t == RW_T_BOOL || t == RW_T_SERIAL || t == RW_T_DATE || t == RW_T_TIME || t == RW_T_TIMESTAMP ||
+           t == RW_T_TIMESTAMPTZ;
+  };
+  if (!is_ordered(a) || !is_ordered(b)) return false;
+  return a == b || (is_int(a) && is_int(b));
+}
+
 int devchunk_from_abi(const rw_chunk* c, DevChunk* out) {
   if (!c || c->n_cols < 0 || c->n_cols > RW_MAX_COLS) return fail(RW_ERR_INVALID, "chunk: bad column count");
   out->n = c->n_rows;

@@ -103,19 +103,14 @@ static int filter_plan(const rw_chunk* c, const rw_filter_term* terms, int32_t n
   if (n_terms < 1 || n_terms > FILTER_MAX_TERMS) return fail(RW_ERR_UNSUPPORTED, "filter: 1..8 conjuncts");
   p->n_terms = n_terms;
   p->upsert = upsert ? 1 : 0;
-  auto int_col = [&](int k) {
-    if (k < 0 || k >= c->n_cols) return false;
-    switch (c->columns[k].type) {
-      case RW_T_BOOL: case RW_T_INT16: case RW_T_INT32: case RW_T_INT64: case RW_T_DATE: case RW_T_TIME:
-      case RW_T_TIMESTAMPTZ: case RW_T_SERIAL: return true;
-      default: return false;
-    }
-  };
   for (int k = 0; k < n_terms; k++) {
     const rw_filter_term& t = terms[k];
     if (t.cmp < RW_CMP_LT || t.cmp > RW_CMP_NE) return fail(RW_ERR_INVALID, "filter: comparison");
-    if (!int_col(t.lhs_col) || (t.rhs_col >= 0 && !int_col(t.rhs_col)) || t.rhs_col < -1)
-      return fail(RW_ERR_UNSUPPORTED, "filter: only integer-typed columns are compared on the device");
+    if (t.lhs_col < 0 || t.lhs_col >= c->n_cols || t.rhs_col < -1 || t.rhs_col >= c->n_cols)
+      return fail(RW_ERR_INVALID, "filter: column index");
+    // a constant right-hand side has the left-hand side's type
+    const int lt = c->columns[t.lhs_col].type, rt = t.rhs_col >= 0 ? c->columns[t.rhs_col].type : lt;
+    if (!cmp_operands_ok(lt, rt)) return fail(RW_ERR_UNSUPPORTED, "filter: operand types the device does not compare stay on the CPU executor");
     p->t[k] = t;
   }
   return RW_OK;
@@ -378,6 +373,8 @@ int32_t rwgpu_filter_device(const rw_chunk* c, const rw_filter_term* terms, int3
   FilterPlanDev p;
   int rc = filter_plan(c, terms, n_terms, upsert, &p);
   if (rc != RW_OK) return rc;
+  // a row reads its neighbours' input ops and visibility while other threads write theirs
+  if (out_ops == c->ops || out_visibility == c->visibility) return fail(RW_ERR_INVALID, "filter: outputs alias the input's ops or visibility");
   DevChunk ch;
   rc = devchunk_from_abi(c, &ch);
   if (rc != RW_OK) return rc;

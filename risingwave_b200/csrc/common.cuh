@@ -35,6 +35,8 @@ int type_width(int t);
 bool type_is_float(int t);
 bool type_is_varlen(int t);
 bool type_supported(int t);
+// the operand rule of join conditions and filter terms (api.cu): may `a cmp b` compare the two raw integers?
+bool cmp_operands_ok(int a, int b);
 
 // ------------------------------------------------------------------ device buffer (RAII)
 struct DevBuf {

@@ -2453,15 +2453,11 @@ int32_t rwgpu_join_create(const rw_join_desc* d, rwgpu_join** out) {
     int ty[2];
     for (int i = 0; i < 2; i++) {
       const int idx = i ? p.cond_rhs : p.cond_lhs;
-      const int t = idx < d->left.n_cols ? d->left.types[idx] : d->right.types[idx - d->left.n_cols];
-      if (type_is_float(t) || t == RW_T_DECIMAL || type_is_varlen(t)) return fail(RW_ERR_UNSUPPORTED, "non-integer join condition stays on the CPU executor");
-      ty[i] = t;
+      ty[i] = idx < d->left.n_cols ? d->left.types[idx] : d->right.types[idx - d->left.n_cols];
     }
-    // cond_ok compares raw integers: int2 / int4 / int8 mix (the reference widens them), every other type only with itself
-    // (date against timestamp would compare days with microseconds; the reference casts the date first)
-    auto is_int = [](int t) { return t == RW_T_INT16 || t == RW_T_INT32 || t == RW_T_INT64; };
-    if (ty[0] != ty[1] && !(is_int(ty[0]) && is_int(ty[1])))
-      return fail(RW_ERR_UNSUPPORTED, "join condition over two different non-integer types stays on the CPU executor");
+    // cond_ok compares raw integers
+    if (!cmp_operands_ok(ty[0], ty[1]))
+      return fail(RW_ERR_UNSUPPORTED, "join condition: operand types the device does not compare stay on the CPU executor");
   }
   p.single_key = (p.n_keys == 1);
   p.KW = p.single_key ? 1 : 1 + p.n_keys;

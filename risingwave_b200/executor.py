@@ -582,10 +582,8 @@ class HashJoinExecutor:
 
 
 # =============================================================================== Filter
-def parse_filter_expr(text: str) -> List[Tuple[int, int, int, int]]:
-    """build_from_pretty subset -> conjunction terms (cmp, lhs_col, rhs_col or -1, rhs_const):
-    `(greater_than:boolean $0:int8 $1:int8)`, `(greater_than:boolean $1:int8 10:int8)`,
-    `(and:boolean (...) (...))`."""
+def _filter_terms(text: str) -> List[Tuple[int, int, int, int, str, str]]:
+    """parse_filter_expr's terms, each with the type annotations of its two operands"""
     text = text.strip()
     m = re.fullmatch(r"\(\s*and:boolean\s+(\(.*\))\s+(\(.*\))\s*\)", text, re.S)
     if m:
@@ -598,13 +596,28 @@ def parse_filter_expr(text: str) -> List[Tuple[int, int, int, int]]:
             if depth == 0:
                 cut = i + 1
                 break
-        return parse_filter_expr(body[:cut]) + parse_filter_expr(body[cut:])
-    m = re.fullmatch(r"\(\s*(\w+):boolean\s+\$(\d+):\w+\s+(?:\$(\d+)|(-?\d+)):\w+\s*\)", text)
+        return _filter_terms(body[:cut]) + _filter_terms(body[cut:])
+    m = re.fullmatch(r"\(\s*(\w+):boolean\s+\$(\d+):(\w+)\s+(?:\$(\d+)|(-?\d+)):(\w+)\s*\)", text)
     if not m or m.group(1) not in _CMP:
         raise ValueError(f"unsupported filter expression {text!r}")
-    if m.group(3) is not None:
-        return [(_CMP[m.group(1)], int(m.group(2)), int(m.group(3)), 0)]
-    return [(_CMP[m.group(1)], int(m.group(2)), -1, int(m.group(4)))]
+    if m.group(4) is not None:
+        return [(_CMP[m.group(1)], int(m.group(2)), int(m.group(4)), 0, m.group(3), m.group(6))]
+    return [(_CMP[m.group(1)], int(m.group(2)), -1, int(m.group(5)), m.group(3), m.group(6))]
+
+
+def parse_filter_expr(text: str) -> List[Tuple[int, int, int, int]]:
+    """build_from_pretty subset -> conjunction terms (cmp, lhs_col, rhs_col or -1, rhs_const):
+    `(greater_than:boolean $0:int8 $1:int8)`, `(greater_than:boolean $1:int8 10:int8)`,
+    `(and:boolean (...) (...))`."""
+    return [t[:4] for t in _filter_terms(text)]
+
+
+# the type names build_from_pretty parses (src/expr/core/src/expr/build.rs:325-340), for the column types a chunk carries
+_FILTER_TYPES = {"boolean": abi.T_BOOL, "int2": abi.T_INT16, "int4": abi.T_INT32, "int8": abi.T_INT64, "serial": abi.T_SERIAL,
+                 "float4": abi.T_FLOAT32, "float8": abi.T_FLOAT64, "decimal": abi.T_DECIMAL, "date": abi.T_DATE,
+                 "time": abi.T_TIME, "timestamp": abi.T_TIMESTAMP, "timestamptz": abi.T_TIMESTAMPTZ,
+                 "varchar": abi.T_VARCHAR, "bytea": abi.T_BYTEA}
+_FILTER_INTS = (abi.T_INT16, abi.T_INT32, abi.T_INT64)
 
 
 _EX_BIN = {"add": abi.EX_ADD, "subtract": abi.EX_SUB, "multiply": abi.EX_MUL, "divide": abi.EX_DIV, "modulus": abi.EX_MOD,
@@ -709,11 +722,19 @@ class FilterExecutor:
 
     def __init__(self, backend: Backend, input: MockSource, expr: str, upsert: bool = False):
         self.backend, self.input, self.upsert = backend, input, upsert
-        terms = parse_filter_expr(expr)
-        self._terms = (abi.RwFilterTerm * len(terms))()
-        for k, (cmp, lhs, rhs, const) in enumerate(terms):
-            self._terms[k].cmp, self._terms[k].lhs_col, self._terms[k].rhs_col, self._terms[k].rhs_const = cmp, lhs, rhs, const
         self.schema = list(input.schema)
+        terms = _filter_terms(expr)
+        self._terms = (abi.RwFilterTerm * len(terms))()
+        for k, (cmp, lhs, rhs, const, lty, rty) in enumerate(terms):
+            # an operand's annotation is its column's type; a constant's is the left operand's, or another integer type
+            # beside an integer one (cmp.rs:44-51 widens them).  The backend sees raw integers and cannot tell.
+            for col, ty in ((lhs, lty), (rhs, rty)):
+                if col >= 0 and (col >= len(self.schema) or _FILTER_TYPES.get(ty) != self.schema[col]):
+                    raise ValueError(f"filter operand ${col}:{ty} does not match the input schema in {expr!r}")
+            lt, ct = _FILTER_TYPES.get(lty), _FILTER_TYPES.get(rty)
+            if rhs < 0 and ct != lt and not (ct in _FILTER_INTS and lt in _FILTER_INTS):
+                raise ValueError(f"filter constant {const}:{rty} does not compare with ${lhs}:{lty} in {expr!r}")
+            self._terms[k].cmp, self._terms[k].lhs_col, self._terms[k].rhs_col, self._terms[k].rhs_const = cmp, lhs, rhs, const
 
     def filter(self, chunk: StreamChunk) -> Optional[StreamChunk]:
         """FilterExecutorInner::filter (filter.rs:58-150): same columns, new ops / visibility; None if no row stays visible"""

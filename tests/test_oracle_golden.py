@@ -137,16 +137,18 @@ def test_filter_golden(oracle, kat):
     run_filter_kat(oracle, kat)
 
 
-def test_filter_oracle_three_valued_and_all_hidden(oracle):
-    """NULL operands make the row's result false (filter.rs:79); a chunk without visible rows yields nothing (:146-150)"""
+def test_filter_oracle_three_valued_all_hidden_and_unpaired_updates(oracle):
+    """NULL operands make the row's result false (filter.rs:79); a chunk without visible rows yields nothing (:146-150); a
+    U- or U+ without its partner follows the project's pairing rule (rwgpu.h) instead of failing the chunk"""
     _, src = MockSource.channel()
     ex = FilterExecutor(oracle, src.into_executor([abi.T_INT64, abi.T_INT64], []),
                         "(and:boolean (greater_than:boolean $0:int8 $1:int8) (less_than:boolean $0:int8 100:int8))")
     got = ex.filter(StreamChunk.from_pretty(" I I\n + 5 . \n + . 1 \n + 7 3 \n + 700 3 \n - 9 8"))
     assert got == StreamChunk.from_pretty(" I I\n + 5 . D\n + . 1 D\n + 7 3 \n + 700 3 D\n - 9 8")
     assert ex.filter(StreamChunk.from_pretty(" I I\n + 1 2 \n - 1 2")) is None
-    with pytest.raises(abi.RwError):  # a U- whose U+ is missing: StreamChunk::with_visibility would panic on the lengths
-        ex.filter(StreamChunk.from_pretty(" I I\n U- 5 1 \n + 7 3"))
+    # a U- whose U+ is missing (the reference never sees one): filtered like a -, keeping its op, as on the device
+    got = ex.filter(StreamChunk.from_pretty(" I I\n U- 5 1 \n U- 50 1 \n + 7 3 \n U- 500 1 \n U+ 5 1"))
+    assert got == StreamChunk.from_pretty(" I I\n U- 5 1 \n U- 50 1 \n + 7 3 \n U- 500 1 D\n + 5 1")
 
 
 def test_nexmark_q4_end_to_end_fixture(oracle):
