@@ -263,8 +263,9 @@ int32_t rwgpu_join_push(rwgpu_join* h, int32_t side, const rw_chunk* chunk, rwgp
 /* DEVICE chunk; output left in HBM as one un-cut chunk `view` (device pointers, valid until the
  * next push on this handle).  *view.n_rows is read back (one 8-byte D2H).
  * ALIASING: when the output is positional (output row r belongs to input row r) the view's columns
- * that are plain copies of `chunk`'s columns may point into `chunk`'s own device buffers instead of
- * a copy.  Keep `chunk`'s buffers alive and unmodified for as long as the view is used: until the
+ * that are plain copies of `chunk`'s columns -- for an inner join on one key column, the matched
+ * side's key column too, which equals the chunk's key -- may point into `chunk`'s own device buffers
+ * instead of a copy.  Keep `chunk`'s buffers alive and unmodified for as long as the view is used: until the
  * next push on this handle (for the _async / collect pair below: until the second _async after
  * the push).  A chunk with a device-resident row count is never aliased.                      */
 int32_t rwgpu_join_push_device(rwgpu_join* h, int32_t side, const rw_chunk* chunk, rw_chunk* view,

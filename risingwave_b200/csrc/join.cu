@@ -1822,16 +1822,16 @@ static int uni_alloc_buckets(rwgpu_join* h, DevBuf& buf, uint64_t cap) {
   return RW_OK;
 }
 
-// keep the load of the bucket array <= 0.5 (every extra probe is one more random 64-byte transaction)
+// keep the load of the bucket array <= 1 / U_LOAD_INV (every extra probe is one more random 64-byte transaction)
 static int uni_grow_table(rwgpu_join* h, uint64_t need_keys) {
-  if (need_keys * 2 <= h->uni_cap) return RW_OK;
+  if (need_keys * U_LOAD_INV <= h->uni_cap) return RW_OK;
   // `need_keys` is an upper bound: every row of every outstanding push counted as a new key, and a push whose row count
   // lives on the device counted at its buffer CAPACITY (N>1: world x the rows it will really hold).  As long as the
-  // keys KNOWN to exist keep the load under 0.5 and even the bound leaves a tenth of the buckets free, probing
+  // keys KNOWN to exist keep the load under the maximum and even the bound leaves a tenth of the buckets free, probing
   // terminates and nothing has to stop; the exact count arrives with the next collect.
-  if (h->uni_keys_exact * 2 <= h->uni_cap && need_keys * 10 <= h->uni_cap * 9) return RW_OK;
+  if (h->uni_keys_exact * U_LOAD_INV <= h->uni_cap && need_keys * 10 <= h->uni_cap * 9) return RW_OK;
   uint64_t ncap = h->uni_cap;
-  while (ncap < need_keys * 4) ncap <<= 1;
+  while (ncap < need_keys * 2 * U_LOAD_INV) ncap <<= 1;  // regrow to half the maximum load
   RW_CUDA(cudaDeviceSynchronize());  // every push in flight on any stream has finished with the old array
   DevBuf nb;
   int rc = uni_alloc_buckets(h, nb, ncap);
@@ -1937,9 +1937,10 @@ static int uni_launch_main(rwgpu_join* h, const JoinPending& pd, bool probe_only
     PlainOut po;
     po.ops = od.ops;
     po.vis = od.vis;
+    const int mkey = pd.alias_u ? h->w8[1 - S].key_col : -1;  // the matched key column equals the input's key column
     for (int c = 0; c < 4; c++) {
       po.ucol[c] = (!pd.alias_u && c < w.n_u && w.u_out[c] >= 0) ? (unsigned long long*)od.col[w.u_out[c]] : nullptr;
-      po.mcol[c] = (c < w.n_m && w.m_out[c] >= 0) ? (unsigned long long*)od.col[w.m_out[c]] : nullptr;
+      po.mcol[c] = (c != mkey && c < w.n_m && w.m_out[c] >= 0) ? (unsigned long long*)od.col[w.m_out[c]] : nullptr;
     }
     po.capacity = od.capacity;
     auto hot = probe_only ? (is_row ? uni_hot_kernel<true, true> : uni_hot_kernel<true, false>)
@@ -2113,6 +2114,9 @@ static int uni_finish(rwgpu_join* h, const JoinPending& pd, int64_t* out_rows, u
     for (int c = 0; c < w.n_u; c++)
       if (w.u_out[c] >= 0)
         RW_CUDA(cudaMemcpyAsync(h->os().out_col[w.u_out[c]].p, pd.ch.cols[c].data, (size_t)pd.ch.n * 8, cudaMemcpyDeviceToDevice, st));
+    const int mk = w.m_out[h->w8[1 - pd.S].key_col];  // (skipped by the hot kernel as well: uni_launch_main)
+    if (mk >= 0)
+      RW_CUDA(cudaMemcpyAsync(h->os().out_col[mk].p, pd.ch.cols[w.key_col].data, (size_t)pd.ch.n * 8, cudaMemcpyDeviceToDevice, st));
   }
   if (aliased) *aliased = alias;
   return RW_OK;
@@ -2509,7 +2513,7 @@ int32_t rwgpu_join_create(const rw_join_desc* d, rwgpu_join** out) {
   if (h->uni) {
     const uint64_t hint = std::max(d->left.row_capacity_hint, d->right.row_capacity_hint);
     uint64_t cap = 1024;
-    while (cap * 4 < hint * 10) cap <<= 1;  // load <= 0.4 at `hint` keys
+    while (cap * 4 < hint * 5 * U_LOAD_INV) cap <<= 1;  // load <= 0.8 of the maximum at `hint` keys
     h->uni_cap = cap;
     rc = uni_alloc_buckets(h, h->uni_buckets, cap);
     if (rc != RW_OK) return rc;
@@ -2696,9 +2700,14 @@ static int join_fill_view(rwgpu_join* h, int64_t n, unsigned long long nullm, rw
       col.validity = h->os().out_bits[k].as<uint64_t>();
     }
   }
-  if (alias_in)
-    for (int c = 0; c < h->w8[S].n_u; c++)
-      if (h->w8[S].u_out[c] >= 0) cols[(size_t)h->w8[S].u_out[c]].data = alias_in->cols[c].data;
+  if (alias_in) {
+    const W8Plan& w = h->w8[S];
+    for (int c = 0; c < w.n_u; c++)
+      if (w.u_out[c] >= 0) cols[(size_t)w.u_out[c]].data = alias_in->cols[c].data;
+    // an inner join's matched key equals the input's key, bit for bit (Key64, non-float): that column aliases it too
+    const int mk = w.m_out[h->w8[1 - S].key_col];
+    if (mk >= 0) cols[(size_t)mk].data = alias_in->cols[w.key_col].data;
+  }
   view->n_rows = n;
   view->n_cols = (int32_t)h->out_types.size();
   view->reserved = 0;

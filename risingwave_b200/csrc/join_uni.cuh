@@ -5,7 +5,7 @@
 // join key owns ONE 64-byte bucket that carries the state of BOTH sides, so a row's probe and its own-side
 // insert touch the SAME line: one random read + one write-back per row, everything else is sequential.
 //
-//   bucket (64 B, linear probing bucket by bucket, load <= 0.5):
+//   bucket (64 B, linear probing bucket by bucket, load <= 1 / U_LOAD_INV = 0.25):
 //     +0   key                 J_EMPTY = free
 //     +8   WI   inline side:   overflow head (31) | inline state (2) | live rows (31)      (as in join.cu)
 //     +16  IH   inline record: null mask (8 bits) | seq << 8
@@ -31,7 +31,13 @@ namespace rw {
 
 #define U_NIL 0x7fffffffu
 #define U_XCHUNK 64  // extra-match output rows a warp reserves at a time
-#define U_MAX_GRID (RW_SMS * 8)  // blocks of JF_BLOCK threads of uni_hot_kernel; one id pool per warp and side
+// blocks of JF_BLOCK threads of uni_hot_kernel, one resident wave (__launch_bounds__(JF_BLOCK, 4)); one id pool per warp
+// and side
+#define U_MAX_GRID (RW_SMS * 4)
+// The bucket array holds at most cap / U_LOAD_INV keys (create-time sizing and uni_grow_table).  At 1/4 (load about 0.15
+// at the create-time hint) a key takes ~1.09 bucket probes instead of ~1.21 at 1/2, and about half the warp iterations
+// wait on a second probe round instead of 85 %; the bucket array is twice as large (64 B x 2^26 = 4 GiB for 10 M keys).
+#define U_LOAD_INV 4
 
 // A side's log is a list of fixed-size SEGMENTS (2^22 records = 192 MiB each) reached through a small device table of
 // segment pointers: growing the log allocates one more segment and appends its pointer -- no copy of the existing

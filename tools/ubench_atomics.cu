@@ -67,12 +67,13 @@ template <int MODE> void run(const char* name, ulonglong2* tab, uint64_t slots, 
 
 int main() {
   unsigned long long* sink; cudaMalloc(&sink, 8);
-  if (getenv("UBENCH_SWEEP")) {  // footprint sweep: where does random access fall off (TLB reach)?
-    for (uint64_t slots : {1ull << 26, 1ull << 27, 1ull << 28, 1ull << 29, 1ull << 30}) {
+  if (getenv("UBENCH_SWEEP")) {  // footprint sweep at the join's bucket-table sizes (1, 2, 4 GiB): TLB reach, DRAM pages
+    for (uint64_t slots : {1ull << 26, 1ull << 27, 1ull << 28}) {
       ulonglong2* tab; if (cudaMalloc(&tab, slots * 16) != cudaSuccess) break; cudaMemset(tab, 0, slots * 16);
       uint64_t n = 1ull << 24;
       run<0>("16B load (ld.cg)", tab, slots, n, sink);
-      run<2>("ATOM.EXCH u32", tab, slots, n, sink);
+      run<12>("load -> store16", tab, slots, n, sink);
+      run<13>("load16 + EXCH64 (+RED if moved)", tab, slots, n, sink);
       cudaFree(tab);
     }
     return 0;
