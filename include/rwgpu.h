@@ -173,8 +173,13 @@ int32_t rwgpu_agg_flush_collect(rwgpu_agg* h, rw_chunk* view, void* cuda_stream)
  *     arguments: the IEEE-754 bits of the f64), one row per live input value of a retractable min / max (0 rows
  *     otherwise).  The shim hands both to StateTable::write_chunk, which does the value / memcomparable encoding and
  *     the vnode prefix (state_table.rs:1451-1560).  Release both with rwgpu_out_release.
- *   rwgpu_agg_restore: into an idle operator; chunks of the same two schemas (HOST).  Afterwards the operator emits
- *     exactly what the snapshotted one would.                                                                     */
+ *   rwgpu_agg_restore: into an idle operator (no push since the last barrier, host pushes still staged included);
+ *     chunks of the same two schemas (HOST), the column types checked before anything is applied.  Afterwards the
+ *     operator emits exactly what the snapshotted one would; a barrier right after a restore emits nothing.  A restore
+ *     may be split over several calls (`minput` may be NULL or empty).  Each minput row must name a retractable
+ *     min / max call (index in [0, n_calls)) of a group whose state row was restored in the same call or an earlier
+ *     one: a row for any other group -- also one whose state row only comes in a later call -- or call is
+ *     RW_ERR_INVALID.  After a refused restore the operator's state is unspecified: drop it.                       */
 int32_t rwgpu_agg_snapshot(rwgpu_agg* h, rwgpu_out** states, rwgpu_out** minput);
 int32_t rwgpu_agg_restore(rwgpu_agg* h, const rw_chunk* states, const rw_chunk* minput);
 /* number of groups currently held / table capacity (diagnostics, join_cached_entry_count-like) */
@@ -312,7 +317,17 @@ int32_t rwgpu_join_stats(rwgpu_join* h, uint64_t* left_rows, uint64_t* right_row
  * derive the output watermarks) and tells the operator which side's state may drop every row whose join key column
  * `key_pos` is below `value` (integer-typed key columns).  Like the reference's state table the rows leave at the next
  * rwgpu_join_barrier.  By the watermark contract no later row can match them, so results are unchanged; the
- * state stops growing.                                                                                     */
+ * state stops growing.  Rules:
+ *  - "below" is the signed order of the column's type (int2 / int4 / date values sign-extended); a row whose key column
+ *    `key_pos` is NULL is never below a watermark (memcomparable sorts NULL last);
+ *  - one watermark per side is pending until the barrier: a lower `value` for the same `key_pos` is ignored, another
+ *    `key_pos` replaces the pending one;
+ *  - late rows (below the watermark after cleaning; the reference leaves their result open): a late insert is an
+ *    ordinary insert and matches nothing of the cleaned side; a late delete of a cleaned row finds no stored row,
+ *    which is RW_ERR_INCONSISTENT under strict_consistency and otherwise changes no state (it still probes the other
+ *    side like any delete);
+ *  - float and bool key columns: RW_ERR_UNSUPPORTED (the state is kept); a bad side or key_pos: RW_ERR_INVALID;
+ *  - on the unified table the cleaned rows count as dead for the rebuild below (rwgpu_join_compactions).          */
 int32_t rwgpu_join_update_watermark(rwgpu_join* h, int32_t side, int32_t key_pos, int64_t value);
 /* ---- state persistence (checkpoint / recovery).  A side's persistent state is the set of its stored input rows: the
  * reference writes every stored row to the side's StateTable (JoinHashMap::insert, join/hash_join.rs:591-625; table
@@ -320,8 +335,12 @@ int32_t rwgpu_join_update_watermark(rwgpu_join* h, int32_t side, int32_t key_pos
  * on to StateTable::write_chunk exactly as the CPU executor does -- nothing has to come back from the GPU.
  *   rwgpu_join_snapshot: the live rows of `side` as all-Insert chunks in the side's input schema (for a checkpoint of
  *     an operator that was running without a StateTable, and for moving state when vnodes are re-assigned).
- *   rwgpu_join_restore: replays state rows (HOST chunk) as inserts with the output discarded -- restore BOTH sides;
- *     the incremental algorithm itself re-derives the degrees of outer / semi / anti joins.                        */
+ *   rwgpu_join_restore: replays state rows (HOST chunk) as inserts with the output discarded -- restore BOTH sides,
+ *     in either order, in one call or several; the incremental algorithm itself re-derives the degrees of outer /
+ *     semi / anti joins.  Of two live rows of one key with an equal pk (an inconsistent stream only: the reference's
+ *     state table, keyed by join key | pk, cannot hold both) restored in one chunk, a later delete removes the later
+ *     one on the unified and fused paths and the earlier one on the generic path -- in neither case necessarily the
+ *     one the snapshotted operator would have removed.                                                          */
 int32_t rwgpu_join_snapshot(rwgpu_join* h, int32_t side, rwgpu_out** rows);
 int32_t rwgpu_join_restore(rwgpu_join* h, int32_t side, const rw_chunk* rows);
 /* State reclamation: a delete marks the stored row dead; rwgpu_join_barrier rebuilds a side's row log from its live

@@ -29,6 +29,7 @@ namespace rw {
 #define AGG_ERR_OUT_CAPACITY 8u
 #define AGG_ERR_MM_MISSING 16u   // retracting a value that is not in the call's materialized input
 #define AGG_ERR_MM_CAPACITY 32u  // internal: materialized-input log full
+#define AGG_ERR_MM_BAD_ROW 64u   // restore: a materialized-input row names no retractable call, or a group without state
 
 struct AggStatus {
   unsigned long long out_rows;
@@ -138,10 +139,15 @@ __device__ __forceinline__ uint64_t find_or_insert_single(const AggTable& t, int
   }
 }
 
-__device__ __forceinline__ uint64_t find_or_insert_multi(const AggTable& t, const AggPlanDev& p, const uint64_t* kw,
-                                                          uint32_t nullmask, bool* created) {
+__device__ __forceinline__ uint64_t multi_hash(const AggPlanDev& p, const uint64_t* kw, uint32_t nullmask) {
   uint64_t h = 0x9e3779b97f4a7c15ull ^ nullmask;
   for (int k = 0; k < p.n_keys; k++) h = mix64(h ^ kw[k]) + 0x9e3779b97f4a7c15ull;
+  return h;
+}
+
+__device__ __forceinline__ uint64_t find_or_insert_multi(const AggTable& t, const AggPlanDev& p, const uint64_t* kw,
+                                                          uint32_t nullmask, bool* created) {
+  const uint64_t h = multi_hash(p, kw, nullmask);
   uint64_t tag = (h & ~0xFFFFull) | ((uint64_t)nullmask << 8) | 1ull;
   uint64_t mask = t.cap - 1;
   uint64_t idx = (h >> 17) & mask;
@@ -956,17 +962,21 @@ __global__ void __launch_bounds__(256) agg_restore_kernel(AggTable t, AggPlanDev
   if (lane_id() == 0 && created_local) atomicAdd(&t.status->n_groups, (unsigned long long)created_local);
 }
 
-// restore of a materialized-input row: (group key | call index | value) -> one record on the group's chain
+// restore of a materialized-input row: (group key | call index | value) -> one record on the group's chain.  The group
+// must already hold its state row (row count > 0): the row is looked up, never inserted, and refused otherwise.
 __global__ void __launch_bounds__(256) agg_restore_minput_kernel(AggTable t, AggPlanDev p, DevChunk ch) {
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < ch.n; r += (int64_t)gridDim.x * blockDim.x) {
-    uint64_t slot;
-    bool created = false;
+    uint64_t slot = ~0ull;
+    const uint64_t mask = t.cap - 1;
     if (p.single_key) {
       const ColRef& kc = ch.cols[0];
       if (col_is_null(kc, r)) slot = t.cap;
       else {
         const uint64_t key = load_key_word(kc, r);
-        slot = key == AGG_EMPTY ? t.cap + 1 : find_or_insert_single(t, p.HW, key, &created);
+        if (key == AGG_EMPTY) slot = t.cap + 1;
+        else
+          for (uint64_t i = mix64(key) & mask; t.hot[i * p.HW] != AGG_EMPTY; i = (i + 1) & mask)
+            if (t.hot[i * p.HW] == key) { slot = i; break; }
       }
     } else {
       uint64_t kw[RW_MAX_KEYS];
@@ -975,10 +985,19 @@ __global__ void __launch_bounds__(256) agg_restore_minput_kernel(AggTable t, Agg
         if (col_is_null(ch.cols[k], r)) { nm |= 1u << k; kw[k] = 0; }
         else kw[k] = load_key_word(ch.cols[k], r);
       }
-      slot = find_or_insert_multi(t, p, kw, nm, &created);
+      const uint64_t h = multi_hash(p, kw, nm);
+      const uint64_t tag = (h & ~0xFFFFull) | ((uint64_t)nm << 8) | 1ull;
+      for (uint64_t i = (h >> 17) & mask; t.hot[i * p.HW] != 0ull; i = (i + 1) & mask) {
+        bool eq = t.hot[i * p.HW] == tag;
+        for (int k = 0; k < p.n_keys && eq; k++) eq = t.hot[i * p.HW + 1 + k] == kw[k];
+        if (eq) { slot = i; break; }
+      }
     }
     const int c = (int)load_i64(ch.cols[p.n_keys], r);
-    if (c < 0 || c >= p.n_calls || p.mm_off[c] < 0) { atomicOr(&t.status->err, AGG_ERR_MM_MISSING); continue; }
+    if (c < 0 || c >= p.n_calls || p.mm_off[c] < 0 || slot == ~0ull || (long long)t.hot[slot * p.HW + p.KW + p.row_count_call] <= 0) {
+      atomicOr(&t.status->err, AGG_ERR_MM_BAD_ROW);
+      continue;
+    }
     const unsigned long long id = atomicAdd(t.mm_next, 1ull);
     if (id >= t.mm_cap) { atomicOr(&t.status->err, AGG_ERR_MM_CAPACITY); continue; }
     uint64_t* cold = t.cold + slot * p.CW;
@@ -1316,6 +1335,7 @@ static int agg_ensure_out(rwgpu_agg* h, int set, int64_t rows) {
 }
 
 static const char* agg_err_msg(unsigned int e) {
+  if (e & AGG_ERR_MM_BAD_ROW) return "materialized-input row of no retractable min/max call, or of a group without a state row";
   if (e & AGG_ERR_OVERFLOW) return "Numeric out of range";
   if (e & AGG_ERR_NEG_COUNT) return "row count should be non-negative";
   if (e & AGG_ERR_RETRACT_APPEND_ONLY) return "attempt to retract on append-only min/max";
@@ -1325,6 +1345,7 @@ static const char* agg_err_msg(unsigned int e) {
   return "unknown";
 }
 static int agg_err_code(unsigned int e) {
+  if (e & AGG_ERR_MM_BAD_ROW) return RW_ERR_INVALID;
   if (e & AGG_ERR_OVERFLOW) return RW_ERR_NUMERIC_OUT_OF_RANGE;
   if (e & (AGG_ERR_NEG_COUNT | AGG_ERR_RETRACT_APPEND_ONLY | AGG_ERR_MM_MISSING)) return RW_ERR_INCONSISTENT;
   return RW_ERR_CUDA;
@@ -1780,11 +1801,17 @@ int32_t rwgpu_agg_snapshot(rwgpu_agg* h, rwgpu_out** states, rwgpu_out** minput)
 
 int32_t rwgpu_agg_restore(rwgpu_agg* h, const rw_chunk* states, const rw_chunk* minput) {
   if (!h || !states) return fail(RW_ERR_INVALID, "null");
-  if (h->n_pending || h->epoch_rows) return fail(RW_ERR_INVALID, "restore into an idle operator only");
+  if (h->n_pending || h->epoch_rows || h->stage[h->cur].rows) return fail(RW_ERR_INVALID, "restore into an idle operator only");
   const AggPlanDev& p = h->plan;
   if (states->n_cols != (int)h->out_types.size()) return fail(RW_ERR_INVALID, "state rows: group key columns followed by one state column per call");
   for (int k = 0; k < states->n_cols; k++)
     if (states->columns[k].type != h->out_types[k]) return fail(RW_ERR_INVALID, "state rows: column type mismatch");
+  if (minput && minput->n_rows > 0) {
+    if (!h->n_retract) return fail(RW_ERR_INVALID, "materialized-input rows for a plan without retractable min/max");
+    bool ok = minput->n_cols == p.n_keys + 2 && minput->columns[p.n_keys].type == RW_T_INT32 && minput->columns[p.n_keys + 1].type == RW_T_INT64;
+    for (int k = 0; ok && k < p.n_keys; k++) ok = minput->columns[k].type == p.key_type[k];
+    if (!ok) return fail(RW_ERR_INVALID, "materialized-input rows: group key columns, int4 call index, int8 value");
+  }
   int rc = agg_ensure_capacity(h, (uint64_t)states->n_rows);
   if (rc != RW_OK) return rc;
   if (states->n_rows > 0) {
@@ -1799,9 +1826,6 @@ int32_t rwgpu_agg_restore(rwgpu_agg* h, const rw_chunk* states, const rw_chunk* 
     h->groups_upper += (uint64_t)states->n_rows;
   }
   if (minput && minput->n_rows > 0) {
-    if (!h->n_retract) return fail(RW_ERR_INVALID, "materialized-input rows for a plan without retractable min/max");
-    if (minput->n_cols != p.n_keys + 2 || minput->columns[p.n_keys].type != RW_T_INT32 || minput->columns[p.n_keys + 1].type != RW_T_INT64)
-      return fail(RW_ERR_INVALID, "materialized-input rows: group key columns, int4 call index, int8 value");
     const uint64_t need = h->mm_upper + (uint64_t)minput->n_rows;
     if (need > h->mm_cap) {
       RW_CUDA(cudaDeviceSynchronize());
