@@ -150,6 +150,20 @@ int32_t rwgpu_agg_push(rwgpu_agg* h, const rw_chunk* chunk);
  * pointer; the rw_chunk/rw_column structs themselves are host memory.  The kernel is enqueued on
  * `cuda_stream` (a cudaStream_t; NULL = the handle's own stream) and the call does not sync.  */
 int32_t rwgpu_agg_push_device(rwgpu_agg* h, const rw_chunk* chunk, void* cuda_stream);
+/* same, for a DEVICE chunk whose row count is produced ON THE DEVICE by earlier work of `cuda_stream` (the exchange,
+ * rwgpu_shuffle_exchange_flat_device): chunk->n_rows is the CAPACITY of its buffers, *n_rows_dev (DEVICE int64) the
+ * rows to apply.  Only rows [0, *n_rows_dev) are read; rows at or past the count are never input (a reused receive
+ * buffer still holds an earlier, larger batch there).  No host round trip between producer and aggregation: the
+ * kernels read the count in place.  Rules:
+ *  - every chunk rwgpu_agg_push_device accepts is accepted (validity and visibility bitmaps, every plan shape);
+ *  - n_rows_dev == NULL behaves exactly like rwgpu_agg_push_device;
+ *  - a count below 0 (the exchange's -1 on failure) or above chunk->n_rows applies nothing, and the next barrier
+ *    (rwgpu_agg_flush* / _collect) returns RW_ERR_INVALID "device row count out of range";
+ *  - the push is charged at its capacity in the operator's host-side bound on the group count: with
+ *    group_capacity_hint >= groups + about two epochs of capacity, steady-state pushes never wait for the device;
+ *  - `chunk`'s buffers and *n_rows_dev stay valid and unmodified until the push's kernels have run on `cuda_stream`
+ *    (record an event after the push; the producer's next write into the same buffer waits for it).               */
+int32_t rwgpu_agg_push_device_counted(rwgpu_agg* h, const rw_chunk* chunk, const int64_t* n_rows_dev, void* cuda_stream);
 /* barrier: emit one +, - or U-/U+ pair per changed group, outputs copied to host. */
 int32_t rwgpu_agg_flush(rwgpu_agg* h, uint64_t epoch, rwgpu_out** out);
 /* barrier with the delta left in HBM: `view` receives DEVICE pointers to one un-cut chunk

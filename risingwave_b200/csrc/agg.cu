@@ -30,6 +30,7 @@ namespace rw {
 #define AGG_ERR_MM_MISSING 16u   // retracting a value that is not in the call's materialized input
 #define AGG_ERR_MM_CAPACITY 32u  // internal: materialized-input log full
 #define AGG_ERR_MM_BAD_ROW 64u   // restore: a materialized-input row names no retractable call, or a group without state
+#define AGG_ERR_BAD_COUNT 128u   // counted push: the device row count is below 0 or above the chunk's capacity
 
 struct AggStatus {
   unsigned long long out_rows;
@@ -89,6 +90,15 @@ __device__ __forceinline__ void mark_dirty(const AggTable& t, uint64_t slot) {
   if (lane == leader) base = atomicAdd(&t.status->n_dirty, (unsigned int)__popc(m));
   base = __shfl_sync(m, base, leader);
   t.dirty_list[base + __popc(m & ((1u << lane) - 1))] = (uint32_t)slot;
+}
+
+// a chunk whose row count lives on the device (chunk_rows): thread 0 of the apply kernel flags a count out of range,
+// which the next barrier reports (chunk_rows makes it no rows: the push applies nothing)
+__device__ __forceinline__ void agg_check_count(const AggTable& t, const DevChunk& ch) {
+  if (ch.n_dev && blockIdx.x == 0 && threadIdx.x == 0) {
+    const int64_t n = *ch.n_dev;
+    if (n < 0 || n > ch.n) atomicOr(&t.status->err, AGG_ERR_BAD_COUNT);
+  }
 }
 
 struct AggOutDev {
@@ -250,7 +260,9 @@ __device__ __forceinline__ void agg_apply_row(const AggTable& t, const AggPlanDe
 // ------------------------------------------------------------------ generic apply kernel (one thread per row)
 __global__ void __launch_bounds__(256) agg_apply_kernel(AggTable t, AggPlanDev p, DevChunk ch, int per_row_flags) {
   unsigned int created_local = 0;
-  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < ch.n; r += (int64_t)gridDim.x * blockDim.x) {
+  agg_check_count(t, ch);
+  // (the count is re-read per row round, an L1 hit: a loop-wide copy costs the kernel register spills)
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < chunk_rows(ch); r += (int64_t)gridDim.x * blockDim.x) {
     uint8_t op = ch.ops[r];
     if (!row_visible(ch, r, op)) continue;
     uint64_t slot;
@@ -287,7 +299,8 @@ __global__ void __launch_bounds__(256) agg_apply_kernel(AggTable t, AggPlanDev p
 // record with that value (the materialized input is a multiset); if it was the group's current extreme the call is
 // flagged and the barrier recomputes the extreme from the live records.
 __global__ void __launch_bounds__(256) agg_mm_delete_kernel(AggTable t, AggPlanDev p, DevChunk ch) {
-  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < ch.n; r += (int64_t)gridDim.x * blockDim.x) {
+  // (a count out of range was flagged by the apply kernel; the count is re-read per row round, as there)
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < chunk_rows(ch); r += (int64_t)gridDim.x * blockDim.x) {
     const uint8_t op = ch.ops[r];
     if (!row_visible(ch, r, op) || !(op == RW_OP_DELETE || op == RW_OP_UPDATE_DELETE)) continue;
     uint64_t slot;
@@ -350,7 +363,9 @@ __global__ void __launch_bounds__(256) agg_apply_fast_kernel(AggTable t, AggPlan
   __shared__ unsigned int s_base;
   unsigned int created_local = 0;
   const int lane = lane_id(), wid = threadIdx.x >> 5;
-  const int64_t npair = (ch.n + 1) >> 1;
+  agg_check_count(t, ch);
+  const int64_t n = chunk_rows(ch);  // grid sized from the capacity: pairs past the count are idle
+  const int64_t npair = (n + 1) >> 1;
   const longlong2* keyv = (const longlong2*)ch.cols[p.key_col[0]].data;
   const unsigned short* opv = (const unsigned short*)ch.ops;
   for (int64_t base = blockIdx.x * (int64_t)blockDim.x; base < npair; base += (int64_t)gridDim.x * blockDim.x) {
@@ -359,7 +374,7 @@ __global__ void __launch_bounds__(256) agg_apply_fast_kernel(AggTable t, AggPlan
     bool first[2] = {false, false};
     if (i < npair) {
       const int64_t r0 = i * 2;
-      const bool two = (r0 + 1 < ch.n);
+      const bool two = (r0 + 1 < n);
       long long k[2];
       uint8_t op[2];
       long long a[NCALLS][2];
@@ -1208,6 +1223,8 @@ static int agg_order(rwgpu_agg* h, cudaStream_t st) {
   return RW_OK;
 }
 
+// A chunk with a device row count (ch.n_dev) is charged at its capacity ch.n in every host-side upper bound (groups,
+// rows, epoch rows, materialized-input records): the kernels clamp the count themselves, nothing is read back.
 static int agg_apply_dev(rwgpu_agg* h, const DevChunk& ch, cudaStream_t st) {
   if (ch.n <= 0) return RW_OK;
   int rc = agg_ensure_capacity(h, (uint64_t)ch.n);
@@ -1335,6 +1352,7 @@ static int agg_ensure_out(rwgpu_agg* h, int set, int64_t rows) {
 }
 
 static const char* agg_err_msg(unsigned int e) {
+  if (e & AGG_ERR_BAD_COUNT) return "device row count out of range";
   if (e & AGG_ERR_MM_BAD_ROW) return "materialized-input row of no retractable min/max call, or of a group without a state row";
   if (e & AGG_ERR_OVERFLOW) return "Numeric out of range";
   if (e & AGG_ERR_NEG_COUNT) return "row count should be non-negative";
@@ -1345,7 +1363,7 @@ static const char* agg_err_msg(unsigned int e) {
   return "unknown";
 }
 static int agg_err_code(unsigned int e) {
-  if (e & AGG_ERR_MM_BAD_ROW) return RW_ERR_INVALID;
+  if (e & (AGG_ERR_MM_BAD_ROW | AGG_ERR_BAD_COUNT)) return RW_ERR_INVALID;
   if (e & AGG_ERR_OVERFLOW) return RW_ERR_NUMERIC_OUT_OF_RANGE;
   if (e & (AGG_ERR_NEG_COUNT | AGG_ERR_RETRACT_APPEND_ONLY | AGG_ERR_MM_MISSING)) return RW_ERR_INCONSISTENT;
   return RW_ERR_CUDA;
@@ -1656,11 +1674,16 @@ int32_t rwgpu_agg_push(rwgpu_agg* h, const rw_chunk* c) {
 }
 
 int32_t rwgpu_agg_push_device(rwgpu_agg* h, const rw_chunk* c, void* cuda_stream) {
+  return rwgpu_agg_push_device_counted(h, c, nullptr, cuda_stream);
+}
+
+int32_t rwgpu_agg_push_device_counted(rwgpu_agg* h, const rw_chunk* c, const int64_t* n_rows_dev, void* cuda_stream) {
   if (!h || !c) return fail(RW_ERR_INVALID, "null");
   if (c->n_cols != (int)h->in_types.size()) return fail(RW_ERR_INVALID, "chunk schema mismatch");
   DevChunk ch;
   int rc = devchunk_from_abi(c, &ch);
   if (rc != RW_OK) return rc;
+  ch.n_dev = n_rows_dev;
   rc = agg_launch_stage(h);  // keep host-staged rows ordered before this chunk
   if (rc != RW_OK) return rc;
   return agg_apply_dev(h, ch, cuda_stream ? (cudaStream_t)cuda_stream : h->stream);

@@ -352,6 +352,14 @@ __device__ __forceinline__ bool bit_get(const uint64_t* w, int64_t i) {
   return w == nullptr || ((w[i >> 6] >> (i & 63)) & 1ull);
 }
 
+// a chunk whose row count lives on the device (e.g. the output of the exchange): clamp the capacity.
+// A count out of range is no rows; the kernel that reads the count first reports it (JERR_BAD_COUNT / AGG_ERR_BAD_COUNT).
+__device__ __forceinline__ int64_t chunk_rows(const DevChunk& ch) {
+  if (!ch.n_dev) return ch.n;
+  const int64_t n = *ch.n_dev;
+  return (n < 0 || n > ch.n) ? 0 : n;
+}
+
 __device__ __forceinline__ bool row_visible(const DevChunk& c, int64_t r, uint8_t op) {
   return op != 0 && (c.vis_bits == nullptr || ((c.vis_bits[r >> 6] >> (r & 63)) & 1ull));
 }

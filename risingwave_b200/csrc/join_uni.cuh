@@ -77,13 +77,6 @@ __device__ __forceinline__ uint8_t* useg_rec(uint8_t* const* segs, uint32_t id) 
 __device__ __forceinline__ UniRec* urec(const UniDev& t, int side, uint32_t id) { return (UniRec*)useg_rec(t.log[side], id); }
 __device__ __forceinline__ uint64_t uhome(uint64_t key, uint64_t mask) { return mix64(key) & mask; }
 
-// a chunk whose row count lives on the device (e.g. the output of the exchange): clamp the capacity.
-// (uni_hot_kernel reports a count out of range; the kernels behind it treat it as no rows.)
-__device__ __forceinline__ int64_t chunk_rows(const DevChunk& ch) {
-  if (!ch.n_dev) return ch.n;
-  const int64_t n = *ch.n_dev;
-  return (n < 0 || n > ch.n) ? 0 : n;
-}
 __device__ __forceinline__ uint64_t shfl64m(unsigned mask, uint64_t v, int src) {
   return (uint64_t)__shfl_sync(mask, (unsigned long long)v, src);
 }

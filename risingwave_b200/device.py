@@ -125,6 +125,41 @@ class DeviceView:
         return int(acc.numel()), int(acc.sum().item()) & ((1 << 64) - 1)
 
 
+class ViewChunk:
+    """Rows [lo, hi) of a DeviceView as a device chunk over the view's own buffers, columns picked and reordered by
+    `cols` (a projection by column pointers: nothing is copied).  This is how an operator's delta left in HBM is sent
+    through the exchange (q4's outer HashAgg regroups the inner HashAgg's delta by `category`).  Valid as long as the
+    view.  A picked column with NULLs keeps its bitmap in `validity`, which the exchange plans refuse (ValueError)."""
+
+    def __init__(self, view: DeviceView, cols: Sequence[int], lo: int = 0, hi: Optional[int] = None):
+        self.view, self.lo = view, lo
+        self.hi = view.n_rows if hi is None else hi
+        assert 0 <= lo <= self.hi <= view.n_rows
+        self.types = [view.col_types[k] for k in cols]
+        self.ptrs = [view.col_ptrs[k] for k in cols]
+        self.validity = [view.valid_ptrs[k] or None for k in cols]
+        self.visibility = view.vis_ptr or None
+
+    def n_rows(self) -> int:
+        return self.hi - self.lo
+
+    def to_abi(self):
+        if self.visibility is not None or any(v is not None for v in self.validity):
+            raise ValueError("a slice of a view with validity / visibility bitmaps is not addressable by row offset")
+        cols = (abi.RwColumn * max(1, len(self.ptrs)))()
+        for k, (p, t) in enumerate(zip(self.ptrs, self.types)):
+            cols[k].type = t
+            cols[k].data = p + self.lo * abi.TYPE_WIDTH[t]
+            cols[k].validity = None
+        ch = abi.RwChunk()
+        ch.n_rows = self.n_rows()
+        ch.n_cols = len(self.ptrs)
+        ch.ops = self.view.ops_ptr + self.lo if self.n_rows() else None
+        ch.visibility = None
+        ch.columns = cols
+        return ch, cols
+
+
 def _d2d(dst: int, src: int, nbytes: int):
     """device-to-device copy ON TORCH'S CURRENT STREAM, so that the tensor operations that follow are ordered behind it.
     (A plain cudaMemcpy runs on the legacy default stream and, device to device, does not wait on the host: kernels torch
@@ -154,6 +189,8 @@ def _lib():
     if not getattr(lib, "_dev_sigs", False):
         lib.rwgpu_agg_push_device.restype = C.c_int32
         lib.rwgpu_agg_push_device.argtypes = [C.c_void_p, C.POINTER(abi.RwChunk), C.c_void_p]
+        lib.rwgpu_agg_push_device_counted.restype = C.c_int32
+        lib.rwgpu_agg_push_device_counted.argtypes = [C.c_void_p, C.POINTER(abi.RwChunk), C.c_void_p, C.c_void_p]
         lib.rwgpu_agg_flush_device.restype = C.c_int32
         lib.rwgpu_agg_flush_device.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(abi.RwChunk), C.c_void_p]
         lib.rwgpu_agg_flush_device_async.restype = C.c_int32
@@ -212,9 +249,15 @@ def _stream_ptr(stream: Optional[torch.cuda.Stream]):
     return C.c_void_p(stream.cuda_stream) if stream is not None else None
 
 
-def agg_push_device(executor, chunk: DeviceChunk, stream: Optional[torch.cuda.Stream] = None):
+def agg_push_device(executor, chunk: DeviceChunk, stream: Optional[torch.cuda.Stream] = None, n_rows_dev: Optional[int] = None):
+    """`n_rows_dev`: device address of an int64 row count produced by earlier work of `stream` (the chunk's
+    tensors are then the capacity); no host round trip between the producer and the aggregation.  The chunk's
+    tensors and the count must stay unchanged until the push's kernels have run on `stream`."""
     ch, keep = chunk.to_abi()
-    _check(_lib().rwgpu_agg_push_device(executor._h, C.byref(ch), _stream_ptr(stream)))
+    if n_rows_dev is None:
+        _check(_lib().rwgpu_agg_push_device(executor._h, C.byref(ch), _stream_ptr(stream)))
+    else:
+        _check(_lib().rwgpu_agg_push_device_counted(executor._h, C.byref(ch), C.c_void_p(n_rows_dev), _stream_ptr(stream)))
 
 
 def agg_flush_device(executor, epoch: int, stream: Optional[torch.cuda.Stream] = None) -> DeviceView:
