@@ -107,7 +107,9 @@ void rwgpu_out_release(rwgpu_out* out);
  * -- is_append_only == 0 -- RETRACTABLE min/max, the reference's MaterializedInput state (minput.rs): the call's
  * non-NULL input values are kept as a chained multiset in HBM; a retraction kills one record, and if it was the
  * group's extreme the barrier recomputes it from the live records.  string_agg / array_agg / DISTINCT / EOWC
- * => RW_ERR_UNSUPPORTED.  (The value log only grows between restarts; 2^31 values per operator.)            */
+ * => RW_ERR_UNSUPPORTED.  (The value log grows between restarts, except that a barrier which cleans state below a
+ * watermark -- rwgpu_agg_update_watermark -- rebuilds it from its live records when more than half of it is dead;
+ * < 2^31 records in use per operator.)                                                                         */
 #define RW_AGG_COUNT 1     /* count(*) when arg_col < 0, else count(col)   general.rs:155-162 */
 #define RW_AGG_SUM 2       /* general.rs:28-41                                                 */
 #define RW_AGG_MIN 3       /* general.rs:91-108 (append-only) / minput.rs (retractable)        */
@@ -196,6 +198,35 @@ int32_t rwgpu_agg_flush_collect(rwgpu_agg* h, rw_chunk* view, void* cuda_stream)
  *     RW_ERR_INVALID.  After a refused restore the operator's state is unspecified: drop it.                       */
 int32_t rwgpu_agg_snapshot(rwgpu_agg* h, rwgpu_out** states, rwgpu_out** minput);
 int32_t rwgpu_agg_restore(rwgpu_agg* h, const rw_chunk* states, const rw_chunk* minput);
+/* Watermark-driven state cleaning (HashAggExecutor passes the watermark on the window column to its state tables,
+ * hash_agg.rs:503-507, which drop the range below it when the epoch commits): the host keeps the watermark derivation
+ * (a watermark on group key `seq` is buffered and emitted after the barrier's delta, hash_agg.rs:628-637, 660-673) and
+ * tells the operator that every group whose key column `key_pos` (a position in group_key_indices) is below `value`
+ * may leave.  By the watermark contract no later row belongs to such a group, so results are unchanged; the state of a
+ * windowed aggregation stops growing.  Rules:
+ *  - when: at the next barrier (rwgpu_agg_flush, _flush_device, _flush_device_async), AFTER that barrier's delta:
+ *    a group below the watermark that changed in the epoch still emits its + / - / U-U+ there, then leaves (the
+ *    reference's flush_data emits first and calls update_watermark at its end).  After that barrier no group whose key
+ *    column `key_pos` is non-NULL and below `value` is held, nor any value record of such a group.  The cleaning is
+ *    enqueued on the barrier's stream behind the delta: an asynchronous barrier stays asynchronous;
+ *  - order: the signed order of the column's type (int2 / int4 / date values sign-extended; int8, time, timestamp,
+ *    timestamptz and serial as they are); a NULL key is never below a watermark (memcomparable sorts NULL last);
+ *  - one watermark is pending at a time: a lower `value` for the same `key_pos` is ignored, another `key_pos` replaces
+ *    the pending one.  rwgpu_agg_restore leaves it pending;
+ *  - float, bool and decimal key columns: RW_ERR_UNSUPPORTED (the state is kept); a bad `key_pos` or a null handle:
+ *    RW_ERR_INVALID;
+ *  - late rows (below the watermark after cleaning; the reference leaves their result open): a row of a cleaned group
+ *    finds no state and is the first row of a new group -- an insert emits + at the next barrier; a retraction makes
+ *    the row count negative (RW_ERR_INCONSISTENT under strict_consistency, else clamped to 0); a retracted min / max
+ *    value is missing from the new group's materialized input (RW_ERR_INCONSISTENT under strict_consistency);
+ *  - a snapshot taken after the barrier holds neither the cleaned groups nor their materialized-input rows;
+ *  - the table keeps its capacity (a spare table of the same size is kept once a cleaning has run); the group count
+ *    rwgpu_agg_stats reports, and the operator's own bound on it, are the count after cleaning.                   */
+int32_t rwgpu_agg_update_watermark(rwgpu_agg* h, int32_t key_pos, int64_t value);
+/* the value log of retractable min / max (diagnostics): records in use (live, retracted and unreachable ones until a
+ * rebuild) and the number of rebuilds so far.  A cleaning barrier rebuilds the log from its live records when more than
+ * half of it and more than 4096 records are dead, so after it: records in use <= 2 x live records + 4096.          */
+int32_t rwgpu_agg_value_log_stats(rwgpu_agg* h, uint64_t* records_in_use, uint64_t* compactions);
 /* number of groups currently held / table capacity (diagnostics, join_cached_entry_count-like) */
 int32_t rwgpu_agg_stats(rwgpu_agg* h, uint64_t* n_groups, uint64_t* capacity, uint64_t* kernel_launches);
 /* device-time accounting of the dominant kernel (the fused group-by + aggregate apply kernel):

@@ -245,11 +245,13 @@ inline std::vector<StreamChunk> take_out(rwgpu_out* out) {
 // ------------------------------------------------------------------------------------ HashAgg
 struct AggCall { int32_t kind, arg_col, ret_type; };
 
+// window_col_idx_in_group_key: the group key leading the intermediate state table's pk (hash_agg.rs:569-570; group key 0
+// in the reference's test helper, agg_executor.rs:157-171): a watermark on it cleans the state below it
 class HashAggExecutor : public Execute {
  public:
   HashAggExecutor(std::shared_ptr<Execute> input, bool is_append_only, std::vector<AggCall> agg_calls, int32_t row_count_index,
-                  std::vector<int32_t> group_key_indices, int32_t chunk_size = 1024)
-      : input_(std::move(input)) {
+                  std::vector<int32_t> group_key_indices, int32_t chunk_size = 1024, int32_t window_col_idx_in_group_key = 0)
+      : input_(std::move(input)), window_seq_(window_col_idx_in_group_key) {
     std::vector<rw_agg_call> calls;
     for (auto& c : agg_calls) calls.push_back(rw_agg_call{c.kind, c.arg_col, c.ret_type, 0});
     rw_agg_desc d{};
@@ -266,9 +268,22 @@ class HashAggExecutor : public Execute {
     check(rwgpu_agg_create(&d, &h_));
     for (int32_t k : group_key_indices) schema_.push_back(input_->schema()[k]);
     for (auto& c : agg_calls) schema_.push_back(c.ret_type);
+    for (size_t seq = 0; seq < group_key_indices.size(); seq++) group_key_seq_[group_key_indices[seq]] = (int32_t)seq;
+    window_col_ = group_key_indices.at((size_t)window_col_idx_in_group_key);
+    buffered_.resize(group_key_indices.size());
   }
   ~HashAggExecutor() override { rwgpu_agg_destroy(h_); }
-  // execute_inner (hash_agg.rs:561-706): chunks are applied, a barrier flushes the deltas and is forwarded
+  // the Message::Watermark arm of execute_inner (hash_agg.rs:628-637): a watermark on a column that is not a group key is
+  // dropped; one on group key `seq` is buffered as `seq` (the later one wins) until the barrier; one on the window
+  // column also cleans the state below it at the next barrier (update_watermark at the end of flush_data, :503-507)
+  void handle_watermark(const Watermark& wm) {
+    auto it = group_key_seq_.find(wm.col_idx);
+    if (it == group_key_seq_.end()) return;
+    if (wm.col_idx == window_col_) check(rwgpu_agg_update_watermark(h_, window_seq_, wm.val));
+    buffered_[(size_t)it->second] = Watermark{it->second, wm.data_type, wm.val};
+  }
+  // execute_inner (hash_agg.rs:561-706): chunks are applied; a barrier flushes the deltas, then the buffered group-key
+  // watermarks go out in seq order, then the barrier (:651-676)
   std::optional<Message> poll_next() override {
     while (true) {
       if (!pending_.empty()) { Message m = std::move(pending_.front()); pending_.pop_front(); return m; }
@@ -282,14 +297,17 @@ class HashAggExecutor : public Execute {
         rwgpu_out* out = nullptr;
         check(rwgpu_agg_flush(h_, b->epoch, &out));  // flush_data
         for (auto& ch : take_out(out)) pending_.emplace_back(std::move(ch));
+        for (auto& w : buffered_)
+          if (w) { pending_.emplace_back(*w); w.reset(); }
         pending_.emplace_back(*b);
       } else {
-        return m;
+        handle_watermark(std::get<Watermark>(*m));
       }
     }
   }
   const std::vector<int32_t>& schema() const override { return schema_; }
   const std::vector<int32_t>& stream_key() const override { return key_; }
+  rwgpu_agg* handle() const { return h_; }  // for diagnostics (rwgpu_agg_stats)
 
  private:
   std::shared_ptr<Execute> input_;
@@ -297,6 +315,9 @@ class HashAggExecutor : public Execute {
   bool first_ = true;
   std::deque<Message> pending_;
   std::vector<int32_t> schema_, key_;
+  int32_t window_seq_ = 0, window_col_ = 0;
+  std::map<int32_t, int32_t> group_key_seq_;  // input column -> group key seq (the last one of a column grouped twice)
+  std::vector<std::optional<Watermark>> buffered_;
 };
 
 // ------------------------------------------------------------------------------------ Filter

@@ -131,6 +131,7 @@ ABI_SYMBOLS = [
     "rwgpu_type_width", "rwgpu_out_num_chunks", "rwgpu_out_num_rows", "rwgpu_out_chunk",
     "rwgpu_out_release", "rwgpu_agg_create", "rwgpu_agg_destroy", "rwgpu_agg_push",
     "rwgpu_agg_push_device", "rwgpu_agg_push_device_counted", "rwgpu_agg_flush", "rwgpu_agg_flush_device", "rwgpu_agg_flush_device_async", "rwgpu_agg_flush_collect", "rwgpu_agg_stats", "rwgpu_agg_profile", "rwgpu_agg_snapshot", "rwgpu_agg_restore",
+    "rwgpu_agg_update_watermark", "rwgpu_agg_value_log_stats",
     "rwgpu_join_create", "rwgpu_join_destroy", "rwgpu_join_push", "rwgpu_join_push_device", "rwgpu_join_push_device_counted", "rwgpu_join_push_device_async", "rwgpu_join_collect", "rwgpu_join_push_async", "rwgpu_join_collect_out",
     "rwgpu_join_barrier", "rwgpu_join_stats", "rwgpu_join_profile", "rwgpu_join_debug_set_seq", "rwgpu_join_snapshot", "rwgpu_join_restore", "rwgpu_join_update_watermark", "rwgpu_join_compactions", "rwgpu_vnode_compute", "rwgpu_dispatch_rewrite_ops",
     "rwgpu_shuffle_partition_device", "rwgpu_shuffle_p2p_region_bytes",

@@ -38,7 +38,7 @@ struct AggStatus {
   unsigned int err;
   unsigned int n_dirty;  // entries of the dirty list
   unsigned int blocks_done;  // flush kernel: blocks that have finished (the last one publishes the status)
-  unsigned int pad;
+  unsigned int mm_dead;      // value-log records retracted or left behind by cleaned groups since the last compaction
 };
 
 struct AggPlanDev {
@@ -299,6 +299,7 @@ __global__ void __launch_bounds__(256) agg_apply_kernel(AggTable t, AggPlanDev p
 // record with that value (the materialized input is a multiset); if it was the group's current extreme the call is
 // flagged and the barrier recomputes the extreme from the live records.
 __global__ void __launch_bounds__(256) agg_mm_delete_kernel(AggTable t, AggPlanDev p, DevChunk ch) {
+  unsigned int kills = 0;  // records this thread retracted: dead for the value-log compaction (agg_mm_compact_kernel)
   // (a count out of range was flagged by the apply kernel; the count is re-read per row round, as there)
   for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < chunk_rows(ch); r += (int64_t)gridDim.x * blockDim.x) {
     const uint8_t op = ch.ops[r];
@@ -345,9 +346,12 @@ __global__ void __launch_bounds__(256) agg_mm_delete_kernel(AggTable t, AggPlanD
         if (p.strict) atomicOr(&t.status->err, AGG_ERR_MM_MISSING);
         continue;
       }
+      kills++;
       if ((long long)__ldcg(t.hot + slot * p.HW + p.KW + c) == v) atomicOr((unsigned long long*)cold, 1ull << (COLD_RECOMPUTE_SHIFT + c));
     }
   }
+  for (int o = 16; o > 0; o >>= 1) kills += __shfl_xor_sync(0xffffffffu, kills, o);
+  if (lane_id() == 0 && kills) atomicAdd(&t.status->mm_dead, kills);
 }
 
 // ------------------------------------------------------------------ fast path: 1 x 8-byte key, no NULLs anywhere,
@@ -542,7 +546,7 @@ __device__ __forceinline__ void agg_publish(AggStatus* st, unsigned int* has_nul
     s.err = __ldcg(&st->err);
     s.n_dirty = __ldcg(&st->n_dirty);
     s.blocks_done = 0;
-    s.pad = 0;
+    s.mm_dead = 0;
     *pub.st_host = s;
     st->out_rows = 0;
     st->n_dirty = 0;
@@ -758,16 +762,38 @@ __global__ void __launch_bounds__(256) agg_flush_kernel(AggTable t, AggPlanDev p
 // a barrier over an epoch without input rows: only the status publication
 __global__ void agg_epilogue_kernel(AggStatus* st, unsigned int* has_null, AggPublish pub) { agg_publish(st, has_null, pub, threadIdx.x); }
 
-// ------------------------------------------------------------------ rehash (growth) kernel
-__global__ void agg_rehash_kernel(AggTable o, AggTable n, AggPlanDev p) {
+// ------------------------------------------------------------------ rehash kernel: growth, and watermark cleaning
+// live (not retracted) value records on the chains of a group's retractable min / max calls
+__device__ __forceinline__ unsigned int mm_live_records(const AggTable& t, const AggPlanDev& p, const uint64_t* cold) {
+  unsigned int n = 0;
+  for (int c = 0; c < p.n_calls; c++) {
+    if (p.mm_off[c] < 0) continue;
+    for (uint32_t id = (uint32_t)cold[p.mm_off[c]]; id != 0u;) {
+      const uint32_t lk = (uint32_t)t.mm_log[id].x;
+      if (!(lk & MM_DEAD)) n++;
+      id = lk & ~MM_DEAD;
+    }
+  }
+  return n;
+}
+
+// wm_key >= 0: the state-table cleaning below a watermark (rwgpu_agg_update_watermark).  A group whose key column wm_key
+// is non-NULL and below `wm` (signed order of the key word: int2 / int4 / date are sign-extended) is not carried over;
+// its live value records become unreachable and are counted dead for the value-log compaction.
+__global__ void agg_rehash_kernel(AggTable o, AggTable n, AggPlanDev p, int wm_key, long long wm) {
   const uint64_t total = o.cap + 2;
-  unsigned int kept = 0;
+  unsigned int kept = 0, lost = 0;
   for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < total; s += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t* oh = o.hot + s * p.HW;
     const uint64_t* oc = o.cold + s * p.CW;
     const bool dirty = (o.dirty[s >> 5] >> (s & 31)) & 1;
     uint64_t dst;
     if (s >= o.cap) {
+      // single-column keys: slot cap + 1 holds the key INT64_MIN (cap, the NULL key, is never below a watermark)
+      if (wm_key >= 0 && p.single_key && s == o.cap + 1 && (long long)AGG_EMPTY < wm) {
+        lost += mm_live_records(o, p, oc);
+        continue;  // (the new table's side slot stays in its initial state)
+      }
       dst = n.cap + (s - o.cap);
     } else {
       uint64_t w0 = oh[0];
@@ -776,6 +802,14 @@ __global__ void agg_rehash_kernel(AggTable o, AggTable n, AggPlanDev p) {
       // from its LRU and deletes their intermediate-state row, agg_group.rs:473-538)
       long long rc = (long long)oh[p.KW + p.row_count_call];
       if (rc == 0 && !(oc[0] & COLD_HAS_PREV) && !dirty) continue;
+      if (wm_key >= 0) {
+        const bool key_null = !p.single_key && ((w0 >> (8 + wm_key)) & 1ull);
+        const long long kv = (long long)(p.single_key ? w0 : oh[1 + wm_key]);
+        if (!key_null && kv < wm) {
+          lost += mm_live_records(o, p, oc);
+          continue;
+        }
+      }
       kept++;
       uint64_t mask = n.cap - 1;
       if (p.single_key) {
@@ -808,8 +842,83 @@ __global__ void agg_rehash_kernel(AggTable o, AggTable n, AggPlanDev p) {
       n.dirty_list[atomicAdd(&n.status->n_dirty, 1u)] = (uint32_t)dst;
     }
   }
-  for (int d = 16; d > 0; d >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, d);
+  for (int d = 16; d > 0; d >>= 1) {
+    kept += __shfl_xor_sync(0xffffffffu, kept, d);
+    lost += __shfl_xor_sync(0xffffffffu, lost, d);
+  }
   if (lane_id() == 0 && kept) atomicAdd(&n.status->n_groups, (unsigned long long)kept);
+  if (lane_id() == 0 && lost) atomicAdd(&n.status->mm_dead, lost);
+}
+
+// ------------------------------------------------------------------ value-log compaction (after a cleaning rebuild)
+// The records of cleaned groups and retracted records are dead weight in mm_log.  At a cleaning barrier the log is
+// rebuilt from the live records of the surviving groups -- like uni_compact for the join's row log -- when more than
+// half of it, and more than AGG_MM_COMPACT_FLOOR records, are dead.  A rebuild costs a walk of the table and of the log,
+// paid for by the dead records it reclaims; without one the log stays within 2 x live + AGG_MM_COMPACT_FLOOR records.
+// The decision is taken on the device (the host never waits for a barrier): every kernel below re-evaluates it from
+// counters none of them changes before agg_clean_finish_kernel.
+#define AGG_MM_COMPACT_FLOOR 4096ull
+struct AggCleanDev {
+  unsigned long long new_next;  // next record id of the log being rebuilt (1 between rebuilds)
+  unsigned long long compactions;
+};
+
+__device__ __forceinline__ bool mm_compact_due(const AggTable& t) {
+  const unsigned long long used = __ldcg(t.mm_next) - 1, dead = __ldcg(&t.status->mm_dead);
+  return 2 * dead > used + AGG_MM_COMPACT_FLOOR;
+}
+
+// one thread per slot: each chain's live records go, contiguous and linked in order, to `dst` (the spare log)
+__global__ void __launch_bounds__(256) agg_mm_compact_kernel(AggTable t, AggPlanDev p, ulonglong2* dst, AggCleanDev* cd) {
+  if (!mm_compact_due(t)) return;
+  for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < t.cap + 2; s += (uint64_t)gridDim.x * blockDim.x) {
+    uint64_t* cold = t.cold + s * p.CW;
+    for (int c = 0; c < p.n_calls; c++) {
+      if (p.mm_off[c] < 0) continue;
+      uint32_t* head = (uint32_t*)(cold + p.mm_off[c]);
+      if (*head == 0u) continue;  // (empty slots too: their cold rows are zero)
+      unsigned int live = 0;
+      for (uint32_t id = *head; id != 0u;) {
+        const uint32_t lk = (uint32_t)t.mm_log[id].x;
+        if (!(lk & MM_DEAD)) live++;
+        id = lk & ~MM_DEAD;
+      }
+      const unsigned long long base = live ? atomicAdd(&cd->new_next, (unsigned long long)live) : 0ull;
+      unsigned long long j = base;
+      for (uint32_t id = *head; id != 0u;) {
+        const ulonglong2 rec = t.mm_log[id];
+        const uint32_t lk = (uint32_t)rec.x;
+        if (!(lk & MM_DEAD)) {
+          dst[j] = make_ulonglong2(j + 1 < base + live ? j + 1 : 0ull, rec.y);
+          j++;
+        }
+        id = lk & ~MM_DEAD;
+      }
+      *head = (uint32_t)base;
+    }
+  }
+}
+
+// the rebuilt records go back to the handle's log (whose address the host keeps)
+__global__ void __launch_bounds__(256) agg_mm_commit_kernel(AggTable t, const ulonglong2* src, const AggCleanDev* cd) {
+  if (!mm_compact_due(t)) return;
+  const unsigned long long n = __ldcg(&cd->new_next);
+  for (unsigned long long i = 1 + blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
+    t.mm_log[i] = src[i];
+}
+
+// one thread: close the rebuild, and publish the group count and the log's next record id AFTER the cleaning to the
+// barrier's pinned status slot (the flush kernel published the count before it), for the host's upper bounds
+__global__ void agg_clean_finish_kernel(AggTable t, AggCleanDev* cd, int compact, AggStatus* st_host, unsigned long long* mm_next_host) {
+  if (compact && mm_compact_due(t)) {
+    *t.mm_next = cd->new_next;
+    t.status->mm_dead = 0;
+    cd->compactions++;
+  }
+  cd->new_next = 1;
+  st_host->n_groups = t.status->n_groups;
+  *mm_next_host = *t.mm_next;
+  __threadfence_system();
 }
 
 // ------------------------------------------------------------------ state persistence (SURVEY 8(f) rank 3)
@@ -1069,6 +1178,15 @@ struct rwgpu_agg {
   int n_retract = 0;
   DevBuf mm_log, mm_next;
   uint64_t mm_cap = 0, mm_upper = 1;
+  uint64_t mm_charged = 0;  // records ever charged to mm_upper by pushes
+  // watermark-driven state cleaning (rwgpu_agg_update_watermark): one pending watermark, applied at the next barrier by
+  // a rebuild into the spare table (same capacity; the two swap) and, when due, a rebuild of the value log through the
+  // spare log.  Both spares are kept once they have been needed.
+  bool wm_pending = false;
+  int wm_key_pos = 0;
+  int64_t wm_value = 0;
+  DevBuf sp_hot, sp_cold, sp_dirty, sp_dlist, mm_spare, clean_dev;
+  uint64_t sp_cap = 0;
   // staging (host pushes)
   AggStage stage[2];
   int cur = 0;
@@ -1087,6 +1205,8 @@ struct rwgpu_agg {
     int set;
     unsigned long long tag;
     uint64_t rows_total;
+    uint64_t mm_charged;
+    bool cleaned;
     cudaStream_t st;
   } pending[2];
   int n_pending = 0;
@@ -1096,7 +1216,7 @@ struct rwgpu_agg {
   // one logical stream of work per handle: a call on another stream than the previous one waits for it on the device
   cudaStream_t last_st = nullptr;
   cudaEvent_t order_ev = nullptr;
-  PinnedBuf status_host;  // per set: AggStatus @0, has_null flags @64, tag @192 (256 bytes each)
+  PinnedBuf status_host;  // per set: AggStatus @0, has_null flags @64, tag @192, mm_next after cleaning @200 (256 bytes each)
   std::shared_ptr<PinnedPool> pool = std::make_shared<PinnedPool>();
   std::vector<rw_column> dev_view_cols;
 
@@ -1169,7 +1289,7 @@ static int agg_ensure_capacity(rwgpu_agg* h, uint64_t incoming) {
   if (rc != RW_OK) return rc;
   RW_CUDA(cudaMemsetAsync(&h->status.as<AggStatus>()->n_groups, 0, sizeof(unsigned long long), h->stream));
   RW_CUDA(cudaMemsetAsync(&h->status.as<AggStatus>()->n_dirty, 0, sizeof(unsigned int), h->stream));
-  agg_rehash_kernel<<<grid_for((int64_t)ot.cap + 2, 256), 256, 0, h->stream>>>(ot, nt, h->plan);
+  agg_rehash_kernel<<<grid_for((int64_t)ot.cap + 2, 256), 256, 0, h->stream>>>(ot, nt, h->plan, -1, 0);
   RW_CUDA(cudaGetLastError());
   h->launches++;
   RW_CUDA(cudaStreamSynchronize(h->stream));  // old buffers are freed below
@@ -1252,6 +1372,7 @@ static int agg_apply_dev(rwgpu_agg* h, const DevChunk& ch, cudaStream_t st) {
       }
     }
     h->mm_upper += (uint64_t)ch.n * (uint64_t)h->n_retract;
+    h->mm_charged += (uint64_t)ch.n * (uint64_t)h->n_retract;
   }
   bool has_nulls = h->n_retract > 0;  // retractable min / max keeps its "state is non-NULL" flags per row
   for (int c : h->used_cols) if (ch.cols[c].valid_bits || ch.cols[c].valid_bytes) has_nulls = true;
@@ -1369,6 +1490,44 @@ static int agg_err_code(unsigned int e) {
   return RW_ERR_CUDA;
 }
 
+// watermark cleaning, enqueued on `st` behind the barrier's delta (nothing is waited for; no allocation once the spares
+// exist): rebuild into the spare table without the groups below the watermark, swap the tables, compact the value log if
+// due, and publish the counts after cleaning to the barrier's status slot `sh`
+static int agg_clean_enqueue(rwgpu_agg* h, cudaStream_t st, uint8_t* sh) {
+  h->wm_pending = false;
+  if (h->sp_cap != h->cap) {
+    int rc = agg_alloc_table(h, h->cap, h->sp_hot, h->sp_cold, h->sp_dirty, h->sp_dlist);
+    if (rc != RW_OK) return rc;
+    h->sp_cap = h->cap;
+  }
+  if (h->n_retract) RW_CUDA(h->mm_spare.reserve((size_t)h->mm_cap * 16));
+  const AggTable ot = h->table();
+  AggTable nt = ot;
+  nt.hot = h->sp_hot.as<uint64_t>(); nt.cold = h->sp_cold.as<uint64_t>(); nt.dirty = h->sp_dirty.as<uint32_t>(); nt.dirty_list = h->sp_dlist.as<uint32_t>();
+  const int g = grid_for((int64_t)h->cap + 2, 256);
+  RW_CUDA(cudaMemsetAsync(nt.dirty, 0, ((h->cap + 2 + 31) / 32) * 4, st));
+  agg_init_kernel<<<g, 256, 0, st>>>(nt, h->plan, 0);
+  RW_CUDA(cudaMemsetAsync(&h->status.as<AggStatus>()->n_groups, 0, sizeof(unsigned long long), st));
+  agg_rehash_kernel<<<g, 256, 0, st>>>(ot, nt, h->plan, h->wm_key_pos, (long long)h->wm_value);
+  RW_CUDA(cudaGetLastError());
+  std::swap(h->hot, h->sp_hot);
+  std::swap(h->cold, h->sp_cold);
+  std::swap(h->dirty, h->sp_dirty);
+  std::swap(h->dirty_list, h->sp_dlist);
+  h->launches += 2;
+  AggCleanDev* cd = h->clean_dev.as<AggCleanDev>();
+  if (h->n_retract) {
+    agg_mm_compact_kernel<<<g, 256, 0, st>>>(nt, h->plan, h->mm_spare.as<ulonglong2>(), cd);
+    agg_mm_commit_kernel<<<grid_for((int64_t)h->mm_cap, 256), 256, 0, st>>>(nt, h->mm_spare.as<ulonglong2>(), cd);
+    RW_CUDA(cudaGetLastError());
+    h->launches += 2;
+  }
+  agg_clean_finish_kernel<<<1, 1, 0, st>>>(nt, cd, h->n_retract ? 1 : 0, (AggStatus*)sh, (unsigned long long*)(sh + 200));
+  RW_CUDA(cudaGetLastError());
+  h->launches++;
+  return RW_OK;
+}
+
 // enqueue the barrier's delta computation on `st` (one launch; nothing is waited for): the rows go to output set
 // h->flip, the status to that set's pinned slot.  At most two barriers may be outstanding.
 static int agg_flush_enqueue(rwgpu_agg* h, cudaStream_t st) {
@@ -1409,12 +1568,19 @@ static int agg_flush_enqueue(rwgpu_agg* h, cudaStream_t st) {
   }
   RW_CUDA(cudaGetLastError());
   h->launches++;
+  const bool cleaned = h->wm_pending;
+  if (cleaned) {
+    rc = agg_clean_enqueue(h, st, sh);
+    if (rc != RW_OK) return rc;
+  }
   if (!h->pend_ev[set]) RW_CUDA(cudaEventCreateWithFlags(&h->pend_ev[set], cudaEventDisableTiming));
   RW_CUDA(cudaEventRecord(h->pend_ev[set], st));
   rwgpu_agg::Pending& pd = h->pending[h->n_pending++];
   pd.set = set;
   pd.tag = pub.tag;
   pd.rows_total = h->rows_total;
+  pd.mm_charged = h->mm_charged;
+  pd.cleaned = cleaned;
   pd.st = st;
   h->flip ^= 1;
   h->epoch_rows = 0;
@@ -1433,7 +1599,9 @@ static int agg_flush_collect(rwgpu_agg* h, int64_t* n_rows, unsigned int* has_nu
   uint8_t* sh = h->status_host.as<uint8_t>() + 256 * pd.set;
   if (*(volatile unsigned long long*)(sh + 192) != pd.tag) return fail(RW_ERR_CUDA, "internal: barrier status was not published");
   AggStatus* s = (AggStatus*)sh;
-  h->groups_upper = s->n_groups + (h->rows_total - pd.rows_total);
+  h->groups_upper = s->n_groups + (h->rows_total - pd.rows_total);  // (after a cleaning: the groups it kept)
+  if (pd.cleaned && h->n_retract)
+    h->mm_upper = std::min<uint64_t>(h->mm_upper, *(volatile unsigned long long*)(sh + 200) + (h->mm_charged - pd.mm_charged));
   *set = pd.set;
   if (s->err) {
     unsigned int e = s->err;
@@ -1586,6 +1754,11 @@ int32_t rwgpu_agg_create(const rw_agg_desc* d, rwgpu_agg** out) {
     const unsigned long long one = 1;  // record ids start at 1 (0 terminates a chain)
     RW_CUDA(cudaMemcpyAsync(h->mm_next.p, &one, 8, cudaMemcpyHostToDevice, h->stream));
     RW_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  {
+    const AggCleanDev cd0 = {1ull, 0ull};
+    RW_CUDA(h->clean_dev.reserve(sizeof(AggCleanDev)));
+    RW_CUDA(cudaMemcpy(h->clean_dev.p, &cd0, sizeof(cd0), cudaMemcpyHostToDevice));
   }
   if (h->n_retract) {
     h->mm_cap = std::max<uint64_t>(1 << 16, d->group_capacity_hint * 4);
@@ -1889,6 +2062,33 @@ int32_t rwgpu_agg_profile(rwgpu_agg* h, int32_t enable, double* ms, uint64_t* la
   h->prof.ms = 0;
   h->prof.n = 0;
   h->prof.on = enable != 0;
+  return RW_OK;
+}
+
+int32_t rwgpu_agg_update_watermark(rwgpu_agg* h, int32_t key_pos, int64_t value) {
+  if (!h) return fail(RW_ERR_INVALID, "null");
+  if (key_pos < 0 || key_pos >= h->plan.n_keys) return fail(RW_ERR_INVALID, "group key position");
+  const int t = h->plan.key_type[key_pos];
+  if (type_is_float(t) || t == RW_T_BOOL || t == RW_T_DECIMAL)
+    return fail(RW_ERR_UNSUPPORTED, "watermarks on this key type keep the state (CPU semantics unchanged)");
+  // a later watermark on the same key only moves up
+  if (!h->wm_pending || value > h->wm_value || key_pos != h->wm_key_pos) {
+    h->wm_pending = true;
+    h->wm_key_pos = key_pos;
+    h->wm_value = value;
+  }
+  return RW_OK;
+}
+
+int32_t rwgpu_agg_value_log_stats(rwgpu_agg* h, uint64_t* records_in_use, uint64_t* compactions) {
+  if (!h) return fail(RW_ERR_INVALID, "null");
+  RW_CUDA(cudaDeviceSynchronize());
+  unsigned long long next = 1;
+  AggCleanDev cd;
+  RW_CUDA(cudaMemcpy(&next, h->mm_next.p, 8, cudaMemcpyDeviceToHost));
+  RW_CUDA(cudaMemcpy(&cd, h->clean_dev.p, sizeof(cd), cudaMemcpyDeviceToHost));
+  if (records_in_use) *records_in_use = next - 1;
+  if (compactions) *compactions = cd.compactions;
   return RW_OK;
 }
 

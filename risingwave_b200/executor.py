@@ -239,11 +239,13 @@ class AggCall:
 # =============================================================================== HashAgg
 class HashAggExecutor:
     """Mirror of HashAggExecutor<K,S> (aggregate/hash_agg.rs); arguments follow
-    `new_boxed_hash_agg_executor` (test_utils/agg_executor.rs:224-300)."""
+    `new_boxed_hash_agg_executor` (test_utils/agg_executor.rs:224-300).  window_col_idx_in_group_key: the group key
+    that leads the intermediate state table's pk (hash_agg.rs:569-570; group key 0 in the reference's test helper,
+    agg_executor.rs:157-171): a watermark on it cleans the state below it."""
 
     def __init__(self, backend: Backend, input: MockSource, is_append_only: bool, agg_calls: Sequence[AggCall],
                  row_count_index: int, group_key_indices: Sequence[int], chunk_size: int = 1024,
-                 strict_consistency: bool = True, group_capacity_hint: int = 0):
+                 strict_consistency: bool = True, group_capacity_hint: int = 0, window_col_idx_in_group_key: int = 0):
         self.backend = backend
         self.input = input
         n_in = len(input.schema)
@@ -271,12 +273,52 @@ class HashAggExecutor:
         backend.check(backend._agg_create(C.byref(d), C.byref(h)))
         self._h = h
         self.schema = [input.schema[k] for k in group_key_indices] + [c.ret_type for c in agg_calls]
+        # watermark derivation (hash_agg.rs:590-597, 628-637): input column -> group key seq (the last seq of a
+        # column that is grouped twice), one buffered watermark per seq
+        self._group_key_seq = {col: seq for seq, col in enumerate(group_key_indices)}
+        self._window_seq = window_col_idx_in_group_key
+        self._window_col = group_key_indices[window_col_idx_in_group_key]
+        self._buffered: List[Optional[Watermark]] = [None] * len(group_key_indices)
 
     def __del__(self):
         h = getattr(self, "_h", None)
         if h:
             self.backend._agg_destroy(h)
             self._h = None
+
+    def handle_watermark(self, wm: Watermark):
+        """the Message::Watermark arm of execute_inner (hash_agg.rs:628-637): a watermark on a column that is not a group
+        key is dropped; one on group key `seq` is buffered as `seq` (the later one wins) until the barrier.  One on the
+        window column also cleans the state below it at the next barrier (the state tables' update_watermark at the end
+        of flush_data, :503-507) -- skipped on a backend without rwgpu_agg_update_watermark, which keeps the state and,
+        under the watermark contract, emits the same rows."""
+        seq = self._group_key_seq.get(wm.col_idx)
+        if seq is None:
+            return
+        if wm.col_idx == self._window_col and hasattr(self.backend.lib, "rwgpu_agg_update_watermark") \
+                and self.backend.prefix == "rwgpu_":
+            self.update_watermark(self._window_seq, wm.val)
+        self._buffered[seq] = Watermark(seq, wm.data_type, wm.val)
+
+    def take_watermarks(self) -> List[Watermark]:
+        """the buffered watermarks in seq order, emitted after a barrier's delta chunks and before the barrier (:660-673)"""
+        out = [w for w in self._buffered if w is not None]
+        self._buffered = [None] * len(self._buffered)
+        return out
+
+    def update_watermark(self, key_pos: int, value: int):
+        """rwgpu_agg_update_watermark: groups whose key column `key_pos` is below `value` leave at the next barrier"""
+        fn = self.backend.lib.rwgpu_agg_update_watermark
+        fn.restype, fn.argtypes = C.c_int32, [C.c_void_p, C.c_int32, C.c_int64]
+        self.backend.check(fn(self._h, key_pos, value))
+
+    def value_log_stats(self) -> Tuple[int, int]:
+        """rwgpu_agg_value_log_stats -> (value-log records in use, rebuilds so far)"""
+        fn = self.backend.lib.rwgpu_agg_value_log_stats
+        fn.restype, fn.argtypes = C.c_int32, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        a, b = C.c_uint64(), C.c_uint64()
+        self.backend.check(fn(self._h, C.byref(a), C.byref(b)))
+        return a.value, b.value
 
     # direct operator calls (what the Rust shim would issue)
     def apply_chunk(self, chunk: StreamChunk):
@@ -312,7 +354,7 @@ class HashAggExecutor:
 
     def _run(self):
         # execute_inner (hash_agg.rs:561-706): first barrier initialises; chunks apply; a barrier
-        # flushes deltas, then is forwarded.
+        # flushes deltas, then the buffered group-key watermarks go out, then the barrier.
         first = True
         while True:
             m = self.input.poll()
@@ -328,9 +370,11 @@ class HashAggExecutor:
                     continue
                 for ch in self.flush_data(m.barrier.epoch):
                     yield Message(chunk=ch)
+                for w in self.take_watermarks():
+                    yield Message(watermark=w)
                 yield m
             else:
-                yield m  # watermarks on group keys pass through (hash_agg.rs:628-637, simplified)
+                self.handle_watermark(m.watermark)
 
 
 # =============================================================================== HashJoin
